@@ -227,9 +227,12 @@ size_t zeggs_speech_enc_workspace_bytes(int B, int T, int C_in, int H, int O);
 int zeggs_speech_enc_fwd(const zeggs_speech_enc_args* a, void* stream);
 int zeggs_speech_enc_bwd(const zeggs_speech_enc_args* a, const zeggs_speech_enc_grads* g, void* stream);
 
-/* StyleEncoder, type "attn", use_vae (modules.py:278-304, 346-420, 484-651): two conv k3 + ReLU + LayerNorm + drop,
+/* StyleEncoder, type "attn" (modules.py:278-304, 346-420, 484-651): two conv k3 + ReLU + LayerNorm + drop,
  * + sinusoidal positions, one FFT block (4-head self-attention + residual LN, 2x conv k3 feed-forward + residual LN),
- * mean over time, mu/logvar split, z = mu + eps * exp(logvar/2) / temperature.
+ * mean over time, then
+ *   use_vae=True  (mu, logvar != NULL): mu/logvar split, z = mu + eps * exp(logvar/2) / temperature; z, mu, logvar [B,E/2];
+ *   use_vae=False (mu == logvar == NULL): z [B,E] = the pooled encoder output (modules.py:303-304); eps is ignored.
+ *     In _bwd, dz is then [B,E] and required, dmu / dlogvar must be NULL.
  * x is the normalised style example [B,T,C_in]; eps [B,E/2] is the N(0,1) sample (NULL = 0); pe [T,E] the
  * positional table; masks are dropout multipliers (NULL = eval): c1 [B,T,H], c2/ao/ff [B,T,E], attn [B,nheads,T,T].
  */
@@ -256,6 +259,40 @@ typedef struct {
 size_t zeggs_style_enc_workspace_bytes(int B, int T, int C_in, int H, int E, int nheads);
 int zeggs_style_enc_fwd(const zeggs_style_enc_args* a, void* stream);
 int zeggs_style_enc_bwd(const zeggs_style_enc_args* a, const zeggs_style_enc_grads* g, void* stream);
+
+/* StyleEncoder, type "gru" (modules.py:278-304, StyleEncoderGRU :307-343): conv k3 (zero pad 1) + ReLU, twice (no LayerNorm, no
+ * dropout), a one-layer bidirectional nn.GRU over the whole example (gate order r, z, n; b_hn inside r * (.)), the projection
+ * LinearNorm(2H -> E) of output[:, -1], then the VAE split and sample exactly as zeggs_style_enc_args describes
+ * (mu == logvar == NULL: z [B,E] = the projection, eps ignored).
+ * Only output[:, -1] is consumed, so the forward direction runs all T steps (one persistent cooperative kernel) while the
+ * reverse direction is the single GRU cell at t = T-1 from h = 0: W_hh_r is not read and dW_hh_r is written as zeros (the
+ * reference's autograd gives it exactly zero).  E = 2 * style_embedding_size with the VAE, style_embedding_size without.
+ * Supported hidden sizes: H % 4 == 0 and H <= 528, or H % 8 == 0 and H <= 1056.  _bwd needs the forward's workspace untouched.
+ */
+typedef struct {
+  int B, T, C_in, H, E;
+  float temperature;
+  const float *Wc1, *bc1;                        /* encoder.convs.0.conv  [H, C_in, 3], [H] */
+  const float *Wc2, *bc2;                        /* encoder.convs.2.conv  [H, H, 3], [H] */
+  const float *W_ih, *W_hh, *b_ih, *b_hh;        /* encoder.rnn_layer.{weight_ih,weight_hh,bias_ih,bias_hh}_l0  [3H,H],[3H,H],[3H],[3H] */
+  const float *W_ih_r, *W_hh_r, *b_ih_r, *b_hh_r; /* the same four with _reverse (W_hh_r is not read) */
+  const float *Wp, *bp;                          /* encoder.projection_layer.linear_layer  [E, 2H], [E] */
+  const float *x, *eps;                          /* [B,T,C_in] normalised example; [B,E/2] N(0,1) sample (NULL = 0) */
+  float *z, *mu, *logvar;                        /* VAE: [B,E/2] each.  Without: z [B,E], mu = logvar = NULL */
+  void* workspace;
+  size_t workspace_bytes;
+  const zeggs_ctx* ctx;
+} zeggs_style_enc_gru_args;
+typedef struct {
+  const float *dz, *dmu, *dlogvar;               /* VAE: [B,E/2], any may be NULL.  Without: dz [B,E] required, dmu = dlogvar = NULL */
+  float *dWc1, *dbc1, *dWc2, *dbc2;
+  float *dW_ih, *dW_hh, *db_ih, *db_hh;
+  float *dW_ih_r, *dW_hh_r, *db_ih_r, *db_hh_r;  /* dW_hh_r: zeros */
+  float *dWp, *dbp;
+} zeggs_style_enc_gru_grads;
+size_t zeggs_style_enc_gru_workspace_bytes(int B, int T, int C_in, int H, int E, int use_vae);
+int zeggs_style_enc_gru_fwd(const zeggs_style_enc_gru_args* a, void* stream);
+int zeggs_style_enc_gru_bwd(const zeggs_style_enc_gru_args* a, const zeggs_style_enc_gru_grads* g, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * One teacher-forced decoder step (RecurrentDecoderNormal.forward, modules.py:179-185), fp32 throughout:

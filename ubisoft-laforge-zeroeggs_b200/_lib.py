@@ -83,6 +83,11 @@ StyleEncArgs = _struct("StyleEncArgs", ints=("B", "T", "C_in", "H", "E", "nheads
                                        "z", "mu", "logvar", "workspace"),
                        tail=[("workspace_bytes", C.c_size_t), ("ctx", C.c_void_p)])
 StyleEncGrads = _struct("StyleEncGrads", ptrs=("dz", "dmu", "dlogvar") + tuple("d" + n for n in STYLE_W))
+STYLE_GRU_W = ("Wc1", "bc1", "Wc2", "bc2", "W_ih", "W_hh", "b_ih", "b_hh", "W_ih_r", "W_hh_r", "b_ih_r", "b_hh_r", "Wp", "bp")
+StyleEncGruArgs = _struct("StyleEncGruArgs", ints=("B", "T", "C_in", "H", "E"), floats=("temperature",),
+                          ptrs=STYLE_GRU_W + ("x", "eps", "z", "mu", "logvar", "workspace"),
+                          tail=[("workspace_bytes", C.c_size_t), ("ctx", C.c_void_p)])
+StyleEncGruGrads = _struct("StyleEncGruGrads", ptrs=("dz", "dmu", "dlogvar") + tuple("d" + n for n in STYLE_GRU_W))
 
 
 DecoderStepArgs = _struct("DecoderStepArgs", ints=("B", "H", "S", "Z"),
@@ -101,7 +106,8 @@ def struct_mirrors():
     return {"zeggs_ctx": Ctx, "zeggs_mel_args": MelArgs, "zeggs_loudness_args": LoudnessArgs, "zeggs_decoder_fwd_args": DecoderFwdArgs,
             "zeggs_decoder_bwd_args": DecoderBwdArgs, "zeggs_speech_enc_args": SpeechEncArgs, "zeggs_speech_enc_grads": SpeechEncGrads,
             "zeggs_style_enc_args": StyleEncArgs, "zeggs_style_enc_grads": StyleEncGrads, "zeggs_decoder_step_args": DecoderStepArgs,
-            "zeggs_loss_args": LossArgs, "zeggs_pose_post_args": PosePostArgs, "zeggs_gather_args": GatherArgs}
+            "zeggs_loss_args": LossArgs, "zeggs_pose_post_args": PosePostArgs, "zeggs_gather_args": GatherArgs,
+            "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads}
 
 
 SYMBOLS = [
@@ -147,6 +153,9 @@ SYMBOLS = [
     ("zeggs_style_enc_workspace_bytes", C.c_size_t, [C.c_int] * 6),
     ("zeggs_style_enc_fwd", C.c_int, [C.POINTER(StyleEncArgs), C.c_void_p]),
     ("zeggs_style_enc_bwd", C.c_int, [C.POINTER(StyleEncArgs), C.POINTER(StyleEncGrads), C.c_void_p]),
+    ("zeggs_style_enc_gru_workspace_bytes", C.c_size_t, [C.c_int] * 6),
+    ("zeggs_style_enc_gru_fwd", C.c_int, [C.POINTER(StyleEncGruArgs), C.c_void_p]),
+    ("zeggs_style_enc_gru_bwd", C.c_int, [C.POINTER(StyleEncGruArgs), C.POINTER(StyleEncGruGrads), C.c_void_p]),
     ("zeggs_loss_workspace_bytes", C.c_size_t, [C.c_int, C.c_int]),
     ("zeggs_loss_fwd_bwd", C.c_int, [C.POINTER(LossArgs), C.c_void_p]),
     ("zeggs_set_fast_wgrad", C.c_int, [C.c_int]),

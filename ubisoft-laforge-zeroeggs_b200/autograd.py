@@ -40,13 +40,15 @@ class SpeechEncoderFn(torch.autograd.Function):
 
 
 class StyleEncoderFn(torch.autograd.Function):
+    """Outputs (z, mu, logvar) with the VAE, z alone without it; either encoder type."""
+
     @staticmethod
     def forward(ctx, enc, x, eps, masks, temperature, *weights):
         outs, ctx.state = ops.style_encoder_fwd(enc, x, eps, masks, temperature)
-        return tuple(outs)
+        return tuple(outs) if outs[1] is not None else outs[0]
 
     @staticmethod
-    def backward(ctx, dz, dmu, dlv):
+    def backward(ctx, dz, dmu=None, dlv=None):
         grads = ops.style_encoder_bwd(ctx.state, dz, dmu, dlv)
         ctx.state = None
         return (None, None, None, None, None) + tuple(grads)

@@ -52,6 +52,14 @@ int sgemm_batched2_launch(int mode, int M, int N, int K, const float* A, int lda
                           const float* bias, float* C, int ldc, int act, int accumulate, int batch,
                           long long sA, long long sB, long long sC, int inner, long long iA, long long iB, long long iC,
                           float alpha, cudaStream_t stream);
+// StyleEncoderGRU recurrences (style_gru.cu)
+int style_gru_units(int H);
+int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
+                         unsigned* bar, cudaStream_t s);
+int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs, const float* Gs, const float* dhf, int ld_dhf,
+                         float* dGih, float* dGhh, unsigned* bar, cudaStream_t s);
+int style_gru_rev_cell_fwd(int B, int H, const float* GIr, const float* bhh, float* hcat, cudaStream_t s);
+int style_gru_rev_cell_bwd(int B, int H, const float* GIr, const float* bhh, const float* dhcat, float* dGIr, float* dGHr, cudaStream_t s);
 
 // units per CTA: the grid G = H/U must fit one CTA per SM (132 on the H100 SXM)
 inline int pick_U(int H) {

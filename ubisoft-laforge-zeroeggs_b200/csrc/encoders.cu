@@ -390,7 +390,9 @@ extern "C" int zeggs_style_enc_fwd(const zeggs_style_enc_args* ap, void* stream_
   ZCHECK_ARG(ap, "style_enc: null args");
   const zeggs_style_enc_args& a = *ap; cudaStream_t s = (cudaStream_t)stream_;
   const int B = a.B, T = a.T, Cin = a.C_in, Hs = a.H, E = a.E, nh = a.nheads, M = B * T, d = E / nh;
-  ZCHECK_ARG(B >= 1 && T >= 1 && nh >= 1 && E % nh == 0 && E % 2 == 0 && a.x && a.z && a.mu && a.logvar, "style_enc: bad arguments");
+  const bool vae = a.mu != nullptr;
+  ZCHECK_ARG(B >= 1 && T >= 1 && nh >= 1 && E % nh == 0 && (!vae || E % 2 == 0) && a.x && a.z && (a.logvar != nullptr) == vae,
+             "style_enc: bad arguments");
   ZCHECK_ARG((long long)B * nh <= 65535, "style_enc: B*nheads too large for one launch");
   StyleWs w = style_ws(a.workspace, B, T, Cin, Hs, E, nh);
   ZCHECK_ARG(a.workspace && a.workspace_bytes >= w.bytes, "style_enc: workspace too small");
@@ -420,6 +422,10 @@ extern "C" int zeggs_style_enc_fwd(const zeggs_style_enc_args* ap, void* stream_
   RC(conv_fwd(w.f1, B, T, E, 3, 1, 0, a.Wf2, a.bf2, w.f2, E, 0, w.colf2, s));
   RC(ew_mul(w.f2d, w.f2, a.mask_ff, nullptr, 0, (size_t)M * E, s));
   RC(ln_fwd(w.f2d, w.x1, a.ln4_g, a.ln4_b, M, E, w.x2, w.xh4, w.rs4, s));                            // :603
+  if (!vae) {                                                                                        // use_vae=False: z = pooled (:303-304)
+    meanpool_kernel<<<ceil_div(B * E, 256), 256, 0, s>>>(w.x2, B, T, E, a.z); LAUNCH_OK();
+    return ZEGGS_OK;
+  }
   meanpool_kernel<<<ceil_div(B * E, 256), 256, 0, s>>>(w.x2, B, T, E, w.pooled); LAUNCH_OK();        // :416-418
   vae_sample_kernel<<<ceil_div(B * (E / 2), 256), 256, 0, s>>>(w.pooled, a.eps, B, E / 2, 1.0f / a.temperature, a.z, a.mu, a.logvar); LAUNCH_OK();
   return ZEGGS_OK;
@@ -433,12 +439,16 @@ extern "C" int zeggs_style_enc_bwd(const zeggs_style_enc_args* ap, const zeggs_s
   StyleWs w = style_ws(a.workspace, B, T, Cin, Hs, E, nh);
   const long long TT = (long long)T * T;
   const size_t nE = (size_t)M * E;
+  const bool vae = a.mu != nullptr;
+  ZCHECK_ARG(vae || (g.dz && !g.dmu && !g.dlogvar), "style_enc bwd: without the VAE (mu == NULL) dz [B,E] is required and dmu / dlogvar must be NULL");
   g_redbuf = w.red;
   RC(colred_reset(s));
   ScopedTimer tm("encoders_bwd", s);
   // VAE sample + mean pool
-  vae_sample_bwd_kernel<<<ceil_div(B * (E / 2), 256), 256, 0, s>>>(g.dz, g.dmu, g.dlogvar, a.eps, a.logvar, B, E / 2, 1.0f / a.temperature, w.pooled); LAUNCH_OK();
-  meanpool_bwd_kernel<<<GRID1(nE), 256, 0, s>>>(w.pooled, B, T, E, w.g0); LAUNCH_OK();               // g0 = d x2
+  if (vae) {
+    vae_sample_bwd_kernel<<<ceil_div(B * (E / 2), 256), 256, 0, s>>>(g.dz, g.dmu, g.dlogvar, a.eps, a.logvar, B, E / 2, 1.0f / a.temperature, w.pooled); LAUNCH_OK();
+  }
+  meanpool_bwd_kernel<<<GRID1(nE), 256, 0, s>>>(vae ? w.pooled : g.dz, B, T, E, w.g0); LAUNCH_OK();  // g0 = d x2
   // x2 = LN4(f2d + x1)
   RC(ln_bwd(w.g0, w.xh4, w.rs4, a.ln4_g, M, E, w.g1, g.dln4_g, g.dln4_b, s));                        // g1 = d(f2d + x1)
   RC(ew_mul(w.g0, w.g1, a.mask_ff, nullptr, 0, nE, s));                                              // g0 = d f2 (pre-act, linear)
@@ -476,6 +486,104 @@ extern "C" int zeggs_style_enc_bwd(const zeggs_style_enc_args* ap, const zeggs_s
   RC(ln_bwd(w.g0, w.xh1, w.rs1, a.ln1_g, M, Hs, w.g1, g.dln1_g, g.dln1_b, s));                       // g1 = d c1
   RC(ew_mul(w.g1, w.g1, nullptr, w.c1, 2, (size_t)M * Hs, s));
   RC(conv_bwd(w.g1, a.x, B, T, Cin, 3, 1, 0, a.Wc1, g.dWc1, g.dbc1, nullptr, Hs, w.col0, s));
+  return ZEGGS_OK;
+}
+
+// ================================================================== StyleEncoder (gru, with or without the VAE)
+// The recurrences are in style_gru.cu; everything around them is the GEMM front end and the small kernels above.
+struct StyleGruWs {
+  unsigned* bar;
+  float *col0, *c1, *col1, *c2, *GI, *Hs, *Gs, *GIr, *hcat, *pooled;
+  float *dpooled, *dhcat, *dGIr, *dGHr, *dGih, *dGhh, *dc2, *dc1, *gcol, *red;   // backward temporaries
+  size_t bytes;
+};
+static StyleGruWs style_gru_ws(void* base, int B, int T, int Cin, int H, int E, bool vae) {
+  Arena a{(char*)base, 0};
+  StyleGruWs w; const size_t R = (size_t)B * T;
+  w.bar = (unsigned*)a.take(64);
+  w.col0 = a.take(R * Cin * 3); w.c1 = a.take(R * H); w.col1 = a.take(R * H * 3); w.c2 = a.take(R * H);
+  w.GI = a.take(R * 3 * H);                    // [B*T][3H] input terms of the forward direction
+  w.Hs = a.take((R + B) * H);                  // [T+1][B][H] h(-1) = 0, h(0) .. h(T-1)
+  w.Gs = a.take(R * 4 * H);                    // [T][B][4H] r, z, n, W_hn h + b_hn
+  w.GIr = a.take((size_t)B * 3 * H); w.hcat = a.take((size_t)B * 2 * H); w.pooled = a.take(vae ? (size_t)B * E : 1);
+  w.dpooled = a.take(vae ? (size_t)B * E : 1); w.dhcat = a.take((size_t)B * 2 * H);
+  w.dGIr = a.take((size_t)B * 3 * H); w.dGHr = a.take((size_t)B * 3 * H);
+  w.dGih = w.GI;                               // GI is dead once the forward recurrence has run: its gradient takes its place
+  w.dGhh = a.take(R * 3 * H);                  // [T][B][3H]
+  w.dc2 = a.take(R * H); w.dc1 = a.take(R * H); w.gcol = a.take(R * H * 3);
+  w.red = a.take((size_t)COLRED_RB * 2 * COLRED_MAXD + COLRED_MAXD / 32);
+  w.bytes = a.off; return w;
+}
+extern "C" size_t zeggs_style_enc_gru_workspace_bytes(int B, int T, int Cin, int H, int E, int use_vae) {
+  if (B < 1 || T < 1 || Cin < 1 || E < 1 || style_gru_units(H) == 0 || (use_vae && E % 2)) return 0;
+  return style_gru_ws(nullptr, B, T, Cin, H, E, use_vae != 0).bytes;
+}
+
+extern "C" int zeggs_style_enc_gru_fwd(const zeggs_style_enc_gru_args* ap, void* stream_) {
+  CtxScope ctx_scope(ap ? ap->ctx : nullptr);
+  ZCHECK_ARG(ap, "style_enc_gru: null args");
+  const zeggs_style_enc_gru_args& a = *ap; cudaStream_t s = (cudaStream_t)stream_;
+  const int B = a.B, T = a.T, Cin = a.C_in, H = a.H, E = a.E, M = B * T;
+  const bool vae = a.mu != nullptr;
+  ZCHECK_ARG(B >= 1 && T >= 1 && Cin >= 1 && E >= 1 && (!vae || E % 2 == 0) && a.x && a.z && (a.logvar != nullptr) == vae,
+             "style_enc_gru: bad arguments");
+  ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru: hidden size %d unsupported (H %% 4 == 0 and H <= 528, or H %% 8 == 0 and H <= 1056)", H);
+  StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);
+  ZCHECK_ARG(a.workspace && a.workspace_bytes >= w.bytes, "style_enc_gru: workspace too small");
+  ScopedTimer tm("encoders_fwd", s);
+  // convs (modules.py:311-333): conv k3 zero-pad -> ReLU, twice
+  RC(conv_fwd(a.x, B, T, Cin, 3, 1, 0, a.Wc1, a.bc1, w.c1, H, 2, w.col0, s));
+  RC(conv_fwd(w.c1, B, T, H, 3, 1, 0, a.Wc2, a.bc2, w.c2, H, 2, w.col1, s));
+  // rnn_layer (:334, 341): forward direction over all T steps, reverse direction = one cell at T-1 from h = 0
+  RC(lin_fwd(w.c2, a.W_ih, a.b_ih, w.GI, M, 3 * H, H, 0, s));
+  RC(style_gru_fwd_launch(B, T, H, a.W_hh, a.b_hh, w.GI, w.Hs, w.Gs, w.hcat, w.bar, s));
+  RC(gemm_f32_auto(0, B, 3 * H, H, w.c2 + (size_t)(T - 1) * H, T * H, a.W_ih_r, H, a.b_ih_r, w.GIr, 3 * H, 0, 0, s));
+  RC(style_gru_rev_cell_fwd(B, H, w.GIr, a.b_hh_r, w.hcat, s));
+  // projection_layer(output[:, -1]) (:342), then the VAE split / sample (:291-302) or z = the projection (:303-304)
+  RC(lin_fwd(w.hcat, a.Wp, a.bp, vae ? w.pooled : a.z, B, E, 2 * H, 0, s));
+  if (vae) {
+    vae_sample_kernel<<<ceil_div(B * (E / 2), 256), 256, 0, s>>>(w.pooled, a.eps, B, E / 2, 1.0f / a.temperature, a.z, a.mu, a.logvar); LAUNCH_OK();
+  }
+  return ZEGGS_OK;
+}
+
+extern "C" int zeggs_style_enc_gru_bwd(const zeggs_style_enc_gru_args* ap, const zeggs_style_enc_gru_grads* gp, void* stream_) {
+  CtxScope ctx_scope(ap ? ap->ctx : nullptr);
+  ZCHECK_ARG(ap && gp, "style_enc_gru bwd: null args");
+  const zeggs_style_enc_gru_args& a = *ap; const zeggs_style_enc_gru_grads& g = *gp; cudaStream_t s = (cudaStream_t)stream_;
+  const int B = a.B, T = a.T, Cin = a.C_in, H = a.H, E = a.E, M = B * T;
+  const bool vae = a.mu != nullptr;
+  ZCHECK_ARG(vae || (g.dz && !g.dmu && !g.dlogvar), "style_enc_gru bwd: without the VAE (mu == NULL) dz [B,E] is required and dmu / dlogvar must be NULL");
+  ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru bwd: hidden size %d unsupported", H);
+  StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);
+  ZCHECK_ARG(a.workspace && a.workspace_bytes >= w.bytes, "style_enc_gru bwd: workspace too small");
+  g_redbuf = w.red;
+  RC(colred_reset(s));
+  ScopedTimer tm("encoders_bwd", s);
+  const float* dproj = g.dz;
+  if (vae) {
+    vae_sample_bwd_kernel<<<ceil_div(B * (E / 2), 256), 256, 0, s>>>(g.dz, g.dmu, g.dlogvar, a.eps, a.logvar, B, E / 2, 1.0f / a.temperature, w.dpooled); LAUNCH_OK();
+    dproj = w.dpooled;
+  }
+  RC(lin_bwd(dproj, w.hcat, a.Wp, g.dWp, g.dbp, w.dhcat, B, E, 2 * H, s));                          // dhcat = d output[:, -1]
+  // reverse cell at T-1: W_ih_r / b_ih_r / b_hh_r gradients, W_hh_r's is zero (it multiplied h = 0)
+  RC(style_gru_rev_cell_bwd(B, H, w.GIr, a.b_hh_r, w.dhcat, w.dGIr, w.dGHr, s));
+  RC(gemm_f32_auto(1, 3 * H, H, B, w.dGIr, 3 * H, w.c2 + (size_t)(T - 1) * H, T * H, nullptr, g.dW_ih_r, H, 0, 0, s));
+  RC(colsum(w.dGIr, B, 3 * H, g.db_ih_r, s));
+  RC(colsum(w.dGHr, B, 3 * H, g.db_hh_r, s));
+  ZCHECK_CUDA(cudaMemsetAsync(g.dW_hh_r, 0, (size_t)3 * H * H * sizeof(float), s));
+  // forward direction: BPTT, then every weight / bias / input gradient as a GEMM or column sum over all (t, b)
+  RC(style_gru_bwd_launch(B, T, H, a.W_hh, w.Hs, w.Gs, w.dhcat, 2 * H, w.dGih, w.dGhh, w.bar, s));
+  RC(gemm_f32_auto(1, 3 * H, H, M, w.dGhh, 3 * H, w.Hs, H, nullptr, g.dW_hh, H, 0, 0, s));            // sum_t dG_hh(t)^T h(t-1)
+  RC(colsum(w.dGhh, M, 3 * H, g.db_hh, s));
+  RC(lin_bwd(w.dGih, w.c2, a.W_ih, g.dW_ih, g.db_ih, w.dc2, M, 3 * H, H, s));
+  RC(gemm_f32_auto(2, B, H, 3 * H, w.dGIr, 3 * H, a.W_ih_r, H, nullptr, w.dc2 + (size_t)(T - 1) * H, T * H, 0, 1, s));   // + reverse cell
+  // convs
+  RC(ew_mul(w.dc2, w.dc2, nullptr, w.c2, 2, (size_t)M * H, s));
+  RC(conv_bwd(w.dc2, w.c1, B, T, H, 3, 1, 0, a.Wc2, g.dWc2, g.dbc2, w.gcol, H, w.col1, s));
+  RC(col2im(w.gcol, B, T, H, 3, 1, 0, w.dc1, s));
+  RC(ew_mul(w.dc1, w.dc1, nullptr, w.c1, 2, (size_t)M * H, s));
+  RC(conv_bwd(w.dc1, a.x, B, T, Cin, 3, 1, 0, a.Wc1, g.dWc1, g.dbc1, nullptr, H, w.col0, s));
   return ZEGGS_OK;
 }
 

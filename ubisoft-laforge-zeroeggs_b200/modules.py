@@ -223,21 +223,48 @@ class StyleEncoderAttn(nn.Module):
         self.blocks = nn.ModuleList([FFTBlock(style_embedding_size)])
 
 
+class StyleEncoderGRU(nn.Module):
+    """Parameter container of modules.py:307-343: conv k3 + ReLU twice, bidirectional one-layer GRU, projection of output[:, -1]."""
+
+    def __init__(self, input_size, hidden_size, style_embedding_size):
+        super().__init__()
+        self.convs = nn.Sequential(
+            ConvNorm1D(input_size, hidden_size, kernel_size=3, stride=1, padding=1, dilation=1, w_init_gain="relu"),
+            nn.ReLU(),
+            ConvNorm1D(hidden_size, hidden_size, kernel_size=3, stride=1, padding=1, dilation=1, w_init_gain="relu"),
+            nn.ReLU())
+        self.rnn_layer = nn.GRU(hidden_size, hidden_size, 1, batch_first=True, bidirectional=True)
+        self.projection_layer = LinearNorm(hidden_size * 2, style_embedding_size, w_init_gain="linear")
+
+
 class StyleEncoder(nn.Module):
-    """modules.py:278-304 (type 'attn').  forward(input[B,T_ex,1134], temprature) -> (z, mu, logvar)."""
+    """modules.py:278-304.  forward(input[B,T_ex,1134], temprature) -> (z, mu, logvar), or (z, None, None) with use_vae=False.
+    type 'attn' (StyleEncoderAttn) or 'gru' (StyleEncoderGRU); the encoder's output size is 2*style_embedding_size with the VAE,
+    style_embedding_size without it.  The type is read off the encoder module, so whole-module pickles of the reference (which
+    store no type) work unchanged."""
 
     def __init__(self, input_size, hidden_size, style_embedding_size, type="attn", use_vae=False):
         super().__init__()
-        if type != "attn":
-            raise _lib.ZeggsError("only the 'attn' style encoder (the shipped configs) is on the accelerated path")
-        if not use_vae:
-            raise _lib.ZeggsError("use_vae=False is not on the accelerated path (the shipped configs use the VAE)")
+        if type not in ("attn", "gru"):
+            raise _lib.ZeggsError(f"unknown style encoder type {type!r} (modules.py:284-287 knows 'attn' and 'gru')")
         self.use_vae = use_vae
         self.style_embedding_size = style_embedding_size
-        self.encoder = StyleEncoderAttn(input_size, hidden_size, 2 * style_embedding_size)
+        output_size = 2 * style_embedding_size if use_vae else style_embedding_size
+        cls = StyleEncoderGRU if type == "gru" else StyleEncoderAttn
+        self.encoder = cls(input_size, hidden_size, output_size)
+
+    @property
+    def encoder_type(self):
+        return "gru" if isinstance(self.encoder, StyleEncoderGRU) else "attn"
 
     def _weights(self):
         e = self.encoder
+        if self.encoder_type == "gru":
+            r = e.rnn_layer
+            return [e.convs[0].conv.weight, e.convs[0].conv.bias, e.convs[2].conv.weight, e.convs[2].conv.bias,
+                    r.weight_ih_l0, r.weight_hh_l0, r.bias_ih_l0, r.bias_hh_l0,
+                    r.weight_ih_l0_reverse, r.weight_hh_l0_reverse, r.bias_ih_l0_reverse, r.bias_hh_l0_reverse,
+                    e.projection_layer.linear_layer.weight, e.projection_layer.linear_layer.bias]
         a, f = e.blocks[0].attention, e.blocks[0].feed_forward
         m = a.multi_head_attention
         return [e.convs[0].conv.weight, e.convs[0].conv.bias, e.convs[2].weight, e.convs[2].bias,

@@ -577,74 +577,132 @@ def style_enc_args(enc, x, eps, masks, temperature, outs, ws):
     if masks is not None:
         for n in ("c1", "c2", "attn", "ao", "ff"):
             setattr(a, "mask_" + n, masks[n].data_ptr())
-    a.z, a.mu, a.logvar = (o.data_ptr() for o in outs)
+    if outs[1] is not None:
+        a.mu, a.logvar = outs[1].data_ptr(), outs[2].data_ptr()
+    a.z = outs[0].data_ptr()
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
     return a, w + [pe]
 
 
+def style_gru_args(enc, x, eps, temperature, outs, ws):
+    dev = x.device
+    w = [_f32c(p, dev) for p in enc._weights()]
+    B, T, Cin = x.shape
+    H, E = w[0].shape[0], w[12].shape[0]
+    a = _lib.StyleEncGruArgs(B=B, T=T, C_in=Cin, H=H, E=E, temperature=temperature, ctx=ctx_ptr(dev))
+    for n, t in zip(_lib.STYLE_GRU_W, w):
+        setattr(a, n, t.data_ptr())
+    a.x = x.data_ptr()
+    if eps is not None:
+        a.eps = eps.data_ptr()
+    if outs[1] is not None:
+        a.mu, a.logvar = outs[1].data_ptr(), outs[2].data_ptr()
+    a.z = outs[0].data_ptr()
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    return a, w
+
+
+def _style_outputs(enc, B, E, dev):
+    """[z, mu, logvar] each [B, E/2] with the VAE; [z [B, E], None, None] without it (modules.py:303-304)."""
+    if enc.use_vae:
+        return [torch.empty((B, E // 2), dtype=torch.float32, device=dev) for _ in range(3)]
+    return [torch.empty((B, E), dtype=torch.float32, device=dev), None, None]
+
+
 def style_encoder_fwd(enc, x, eps, masks, temperature):
-    """zeggs_style_enc_fwd -> ([z, mu, logvar], state for style_encoder_bwd)."""
+    """zeggs_style_enc_fwd (attn) / zeggs_style_enc_gru_fwd (gru) -> ([z, mu, logvar], state for style_encoder_bwd);
+    mu = logvar = None without the VAE."""
     l = _lib.lib()
     x = _f32c(x)
     weights = enc._weights()
     B, T, Cin = x.shape
+    if enc.encoder_type == "gru":
+        H, E = weights[0].shape[0], weights[12].shape[0]
+        outs = _style_outputs(enc, B, E, x.device)
+        nb = l.zeggs_style_enc_gru_workspace_bytes(B, T, Cin, H, E, int(bool(enc.use_vae)))
+        if nb == 0:
+            raise _lib.ZeggsError(f"GRU style encoder: hidden size {H} / encoding size {E} unsupported")
+        ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
+        a, keep = style_gru_args(enc, x, eps, temperature, outs, ws)
+        _lib.check(l.zeggs_style_enc_gru_fwd(a, _lib.stream_ptr()), "zeggs_style_enc_gru_fwd")
+        return outs, ("gru", a, keep, x, eps, masks, outs, ws, weights)
     Hs, E = weights[0].shape[0], weights[4].shape[0]
     nh = enc.encoder.blocks[0].attention.multi_head_attention.num_heads
-    outs = [torch.empty((B, E // 2), dtype=torch.float32, device=x.device) for _ in range(3)]
+    outs = _style_outputs(enc, B, E, x.device)
     ws = torch.empty(l.zeggs_style_enc_workspace_bytes(B, T, Cin, Hs, E, nh), dtype=torch.uint8, device=x.device)
     a, keep = style_enc_args(enc, x, eps, masks, temperature, outs, ws)
     _lib.check(l.zeggs_style_enc_fwd(a, _lib.stream_ptr()), "zeggs_style_enc_fwd")
-    return outs, (a, keep, x, eps, masks, outs, ws, weights)
+    return outs, ("attn", a, keep, x, eps, masks, outs, ws, weights)
 
 
 def style_encoder_bwd(state, dz, dmu, dlv, grads_out=None):
-    a, keep, x, eps, masks, outs, ws, weights = state
+    kind, a, keep, x, eps, masks, outs, ws, weights = state
     a.ctx = ctx_ptr(x.device)              # the lane this call is issued from (may differ from the forward's)
-    g = _lib.StyleEncGrads()
+    g = _lib.StyleEncGruGrads() if kind == "gru" else _lib.StyleEncGrads()
     hold = []
     for n, t in (("dz", dz), ("dmu", dmu), ("dlogvar", dlv)):
         if t is not None:
             t = t.contiguous().float()
             hold.append(t)
             setattr(g, n, t.data_ptr())
+    if outs[1] is None and dz is None:     # without the VAE z is the only output: the library needs its gradient
+        dz = torch.zeros_like(outs[0])
+        hold.append(dz)
+        g.dz = dz.data_ptr()
     grads = _grad_targets(weights, grads_out)
-    for n, t in zip(_lib.STYLE_W, grads):
+    for n, t in zip(_lib.STYLE_GRU_W if kind == "gru" else _lib.STYLE_W, grads):
         setattr(g, "d" + n, t.data_ptr())
-    _lib.check(_lib.lib().zeggs_style_enc_bwd(a, g, _lib.stream_ptr()), "zeggs_style_enc_bwd")
+    if kind == "gru":
+        _lib.check(_lib.lib().zeggs_style_enc_gru_bwd(a, g, _lib.stream_ptr()), "zeggs_style_enc_gru_bwd")
+    else:
+        _lib.check(_lib.lib().zeggs_style_enc_bwd(a, g, _lib.stream_ptr()), "zeggs_style_enc_bwd")
     return grads
 
 
+def _draw_eps(shape, dev):
+    if _dev_seed is not None:                               # device-seeded draw (replayable graph), else torch's generator
+        eps = torch.empty(shape, dtype=torch.float32, device=dev)
+        _dev_seed.salt += 1
+        _lib.check(_lib.lib().zeggs_randn_dev(eps.data_ptr(), eps.numel(), _dev_seed.t.data_ptr(), _dev_seed.salt, _lib.stream_ptr()),
+                   "zeggs_randn_dev")
+        return eps
+    return torch.randn(shape, device=dev)                   # modules.py:299
+
+
 def style_encoder_prepare(enc, x, eps=None, masks=None):
-    """VAE noise (modules.py:299) and dropout multipliers (sampled in train mode unless injected) -> (eps, masks)."""
+    """VAE noise (modules.py:299; drawn only with use_vae) and dropout multipliers (attn encoder only: StyleEncoderGRU has no
+    dropout; sampled in train mode unless injected) -> (eps or None, masks or None)."""
     dev = x.device
     ensure_scratch(dev)
     B, T = x.shape[0], x.shape[1]
-    Hs = enc.encoder.convs[0].conv.weight.shape[0]
-    E = enc.encoder.convs[4].conv.weight.shape[0]
-    nh = enc.encoder.blocks[0].attention.multi_head_attention.num_heads
-    if eps is None:
-        if _dev_seed is not None:                           # device-seeded draw (replayable graph), else torch's generator
-            eps = torch.empty((B, E // 2), dtype=torch.float32, device=dev)
-            _dev_seed.salt += 1
-            _lib.check(_lib.lib().zeggs_randn_dev(eps.data_ptr(), eps.numel(), _dev_seed.t.data_ptr(), _dev_seed.salt, _lib.stream_ptr()),
-                       "zeggs_randn_dev")
-        else:
-            eps = torch.randn((B, E // 2), device=dev)      # modules.py:299
-    if masks is None and enc.training:
-        masks = dict(c1=_drop_mask((B, T, Hs), 0.2, dev), c2=_drop_mask((B, T, E), 0.2, dev),
-                     attn=_drop_mask((B, nh, T, T), 0.1, dev), ao=_drop_mask((B, T, E), 0.1, dev),
-                     ff=_drop_mask((B, T, E), 0.1, dev))
-    if masks is not None:
-        masks = {k: _f32c(v, dev) for k, v in masks.items()}
-    return _f32c(eps, dev), masks
+    gru = enc.encoder_type == "gru"
+    E = (enc.encoder.projection_layer.linear_layer.weight if gru else enc.encoder.convs[4].conv.weight).shape[0]
+    if not enc.use_vae:
+        eps = None
+    elif eps is None:
+        eps = _draw_eps((B, E // 2), dev)
+    if gru:
+        masks = None
+    else:
+        Hs = enc.encoder.convs[0].conv.weight.shape[0]
+        nh = enc.encoder.blocks[0].attention.multi_head_attention.num_heads
+        if masks is None and enc.training:
+            masks = dict(c1=_drop_mask((B, T, Hs), 0.2, dev), c2=_drop_mask((B, T, E), 0.2, dev),
+                         attn=_drop_mask((B, nh, T, T), 0.1, dev), ao=_drop_mask((B, T, E), 0.1, dev),
+                         ff=_drop_mask((B, T, E), 0.1, dev))
+        if masks is not None:
+            masks = {k: _f32c(v, dev) for k, v in masks.items()}
+    return (None if eps is None else _f32c(eps, dev)), masks
 
 
 def style_encoder(enc, x, temperature=1.0, eps=None, masks=None):
+    """-> (z, mu, logvar); (z, None, None) without the VAE, as modules.py:303-304 returns."""
     if x.device.type != "cuda":
         raise _lib.ZeggsError("zeggs_b200.StyleEncoder runs on CUDA tensors only (no CPU fallback)")
     from .autograd import StyleEncoderFn
     eps, masks = style_encoder_prepare(enc, x, eps, masks)
-    return StyleEncoderFn.apply(enc, x, eps, masks, temperature, *enc._weights())
+    out = StyleEncoderFn.apply(enc, x, eps, masks, temperature, *enc._weights())
+    return tuple(out) if enc.use_vae else (out, None, None)
 
 
 # ---------------------------------------------------------------------------------------------- pose -> BVH channel values

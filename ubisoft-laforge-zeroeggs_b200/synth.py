@@ -26,8 +26,9 @@ def _u(rs, shape, bound):
     return rs.uniform(-bound, bound, size=shape).astype(np.float32)
 
 
-def make_params(H=1024, S=64, Z=64, style_hidden=512, style_embed=128, seed=1234, with_style=True):
-    """Random weights with PyTorch-default-like scales for every tensor on the path."""
+def make_params(H=1024, S=64, Z=64, style_hidden=512, style_embed=128, seed=1234, with_style=True, style_type="attn"):
+    """Random weights with PyTorch-default-like scales for every tensor on the path.  style_embed is the style encoder's
+    output size (2*Z with the VAE, Z without); style_type 'attn' (StyleEncoderAttn) or 'gru' (StyleEncoderGRU)."""
     rs = np.random.RandomState(seed)
     A = P_IN + S + Z
     P = {}
@@ -60,7 +61,20 @@ def make_params(H=1024, S=64, Z=64, style_hidden=512, style_embed=128, seed=1234
     P[c + "layer1.bias"] = _u(rs, (H,), kb)
     P[c + "layer2.weight"] = _u(rs, (2 * H, H), kb)
     P[c + "layer2.bias"] = _u(rs, (2 * H,), kb)
-    if with_style:
+    if with_style and style_type == "gru":
+        E, Hs = style_embed, style_hidden
+        e = "style_encoder.encoder."
+        xav = lambda co, ci, k, gain: gain * np.sqrt(6.0 / (ci * k + co * k))
+        P[e + "convs.0.conv.weight"] = _u(rs, (Hs, P_IN, 3), xav(Hs, P_IN, 3, np.sqrt(2)))
+        P[e + "convs.0.conv.bias"] = _u(rs, (Hs,), 1 / np.sqrt(P_IN * 3))
+        P[e + "convs.2.conv.weight"] = _u(rs, (Hs, Hs, 3), xav(Hs, Hs, 3, np.sqrt(2)))
+        P[e + "convs.2.conv.bias"] = _u(rs, (Hs,), 1 / np.sqrt(Hs * 3))
+        for sfx in ("", "_reverse"):                               # nn.GRU default init U(-1/sqrt(H), 1/sqrt(H))
+            for n, shape in (("weight_ih", (3 * Hs, Hs)), ("weight_hh", (3 * Hs, Hs)), ("bias_ih", (3 * Hs,)), ("bias_hh", (3 * Hs,))):
+                P[e + f"rnn_layer.{n}_l0{sfx}"] = _u(rs, shape, 1 / np.sqrt(Hs))
+        P[e + "projection_layer.linear_layer.weight"] = _u(rs, (E, 2 * Hs), np.sqrt(6.0 / (2 * Hs + E)))
+        P[e + "projection_layer.linear_layer.bias"] = _u(rs, (E,), 1 / np.sqrt(2 * Hs))
+    elif with_style:
         E = style_embed  # = 2*Z with use_vae (modules.py:283)
         e = "style_encoder.encoder."
         xav = lambda co, ci, k, gain: gain * np.sqrt(6.0 / (ci * k + co * k))

@@ -1,6 +1,6 @@
 """Training on the GPU path.  `train()` keeps the reference's call surface (ZEGGS/train.py:29-36, called from
 main.py:64-71); `TrainStep` is the step body (train.py:196-432) with every stage running in libzeggs_b200.so:
-speech encoder, style encoder (VAE), persistent decoder window (fwd + BPTT), fused FK/L1 loss, fused RAdam,
+speech encoder, style encoder (attn or gru, VAE on or off), persistent decoder window (fwd + BPTT), fused FK/L1 loss, fused RAdam,
 and -- when torch.distributed is initialised -- ONE NCCL all-reduce of the flat gradient per step.
 """
 import datetime
