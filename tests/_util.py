@@ -46,3 +46,22 @@ def report(name, got, ref):
     scale = float(ref.abs().max())
     print(f"  [{name}] max-abs err {err:.3e} (ref max {scale:.3e})")
     return err, scale
+
+
+def run_with_grads(fn, P, win, speech, style, cot, **kw):
+    """float64 forward of fn (model_oracle.decoder_forward signature) + autograd of sum(out * cot) -> (outputs, {name: gradient}).
+    Gradients the outputs do not depend on are zero."""
+    st = stats_tensors()
+    Pt = {k: torch.from_numpy(v).double().requires_grad_(k.startswith("decoder.")) for k, v in P.items()}
+    sp, sy = speech.double().requires_grad_(True), style.double().requires_grad_(True)
+    out = fn(Pt, *[win[n][:, 0].double() for n in NAMES], win["gaze_pos"].double(), sp, sy,
+             *[st[k].double() for k in ("anim_input_mean", "anim_input_std", "anim_output_mean", "anim_output_std")], st["dt"], **kw)
+    keys = sorted(k for k in Pt if k.startswith("decoder."))
+    leaves = [Pt[k] for k in keys] + [sp, sy]
+    loss = sum((o * c.double()).sum() for o, c in zip(out, cot))
+    if loss.requires_grad:
+        gs = torch.autograd.grad(loss, leaves, allow_unused=True)
+    else:
+        gs = [None] * len(leaves)
+    grads = {k: (g if g is not None else torch.zeros_like(x)) for k, g, x in zip(keys + ["speech", "style"], gs, leaves)}
+    return [o.detach() for o in out], grads

@@ -441,6 +441,31 @@ def test_gemm_f32_splitk_epilogue(dev):
     assert err <= 4e-5 * sc
 
 
+@pytest.mark.parametrize("M,N,K", [(32, 300, 4096), (256, 700, 384)])        # split-K (few output tiles, long K) / not split
+@pytest.mark.parametrize("mode", [0, 1, 2])
+def test_gemm_f32_epilogue_every_operand_layout(dev, mode, M, N, K):
+    """bias + ELU + accumulate epilogue of the split-bf16 GEMM front end in every operand layout (mode 0: A[M,K] B[N,K]^T -- the tc
+    engine's hoisted cond terms --, 1: A[K,M]^T B[K,N] -- its fold matrix --, 2: A[M,K] B[K,N]), with and without split-K: <= 4e-5
+    relative to max|C| vs float64.  The call carries its own zeggs_ctx (GEMM mode 1, fast_wgrad off), so the result does not depend on
+    which decoder engine the process has selected: with the tensor-core engine the shared context runs mode-1 products as ONE bf16 pass."""
+    import ctypes as C
+    from zeggs_b200 import _lib
+    scratch = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    ctx = _lib.Ctx(scratch=scratch.data_ptr(), scratch_bytes=scratch.numel(), gemm_mode=1, fast_wgrad=0)
+    g = torch.Generator().manual_seed(5 + mode)
+    A = torch.randn(K, M, generator=g) if mode == 1 else torch.randn(M, K, generator=g)
+    B = torch.randn(N, K, generator=g) if mode == 0 else torch.randn(K, N, generator=g)
+    bias, C0 = torch.randn(N, generator=g), torch.randn(M, N, generator=g)
+    prod = A.double().T if mode == 1 else A.double()
+    prod = prod @ (B.double().T if mode == 0 else B.double())
+    ref = C0.double() + torch.nn.functional.elu(prod + bias.double())
+    Ad, Bd, bd, out = A.to(dev), B.to(dev), bias.to(dev), C0.to(dev).clone()
+    _lib.check(_lib.lib().zeggs_gemm_f32_ctx(C.addressof(ctx), mode, M, N, K, Ad.data_ptr(), Ad.stride(0), Bd.data_ptr(), Bd.stride(0),
+                                             bd.data_ptr(), out.data_ptr(), N, 1, 1, _lib.stream_ptr()), "zeggs_gemm_f32_ctx")
+    err, sc = report(f"gemm_f32 mode{mode} {M}x{N}x{K} bias+elu+accumulate", out, ref)
+    assert err <= 4e-5 * sc
+
+
 # ---------------------------------------------------------------------------------------------- inference path (config 1)
 def test_generate_motion_end_to_end_vs_oracle(dev):
     """WAV samples -> mel -> SpeechEncoder -> StyleEncoder (example) -> free-running decoder (B=1, 3 s clip), eval mode.
@@ -712,7 +737,7 @@ def test_full_size_tc_forward_vs_oracle(dev, decoder_engine):
 
 @pytest.mark.parametrize("tag", ["h384", "h1024"])
 def test_train_step_tc_engine_vs_reference_golden(dev, golden_dir, decoder_engine, tag):
-    """The whole step body on the TENSOR-CORE engine (H >= 288: U=4/G=96 at H=384, U=8/G=128 -- the bench geometry -- at H=1024)
+    """The whole step body on the TENSOR-CORE engine (H >= 384: U=4/G=96 at H=384, U=8/G=128 -- the bench geometry -- at H=1024)
     against the unmodified reference's loss, 18 terms and gradients (oracle/make_golden.py): loss within 5e-3 relative, terms
     within 3e-2, gradient norms within 5e-2, stored gradient tensors rel-L2 <= 6e-2 (bf16 MMA operands; encoders' weight
     gradients single-pass bf16)."""

@@ -26,6 +26,14 @@ const char* get_error();
     }                                              \
   } while (0)
 
+#define ZCHECK_SUPPORTED(cond, ...)                \
+  do {                                             \
+    if (!(cond)) {                                 \
+      zeggs::set_error(__VA_ARGS__);               \
+      return ZEGGS_ERR_UNSUPPORTED;                \
+    }                                              \
+  } while (0)
+
 #define ZCHECK_CUDA(expr)                                                                 \
   do {                                                                                    \
     cudaError_t _e = (expr);                                                              \

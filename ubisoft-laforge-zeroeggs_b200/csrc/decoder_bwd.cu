@@ -488,7 +488,21 @@ extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const 
   const zeggs_decoder_bwd_args& b = *bp;
   cudaStream_t stream = (cudaStream_t)stream_;
   ZCHECK_ARG(a.save_for_backward && a.workspace, "decoder bwd: forward must have run with save_for_backward=1");
-  ZCHECK_ARG(a.T >= 2, "decoder bwd: T must be >= 2");
+  ZCHECK_ARG(a.T >= 1 && b.phase >= 0 && b.phase <= 2, "decoder bwd: bad T=%d / phase=%d", a.T, b.phase);
+  if (a.T == 1) {
+    // a one-frame window outputs the given first pose (modules.py:72-79): no weight and no conditioning input reaches it, so every
+    // gradient is zero (the reference's autograd gives the same)
+    if (b.phase == 2) return ZEGGS_OK;
+    const size_t H = a.H, A = P_IN + a.S + a.Z, Kin = P_IN + a.Z;
+    const struct { float* p; size_t n; } zero[] = {
+        {b.dW0, H * A}, {b.db0, H}, {b.dW_ih0, 3 * H * (A + H)}, {b.db_ih0, 3 * H}, {b.dW_hh0, 3 * H * H}, {b.db_hh0, 3 * H},
+        {b.dW_ih1, 3 * H * H}, {b.db_ih1, 3 * H}, {b.dW_hh1, 3 * H * H}, {b.db_hh1, 3 * H}, {b.dW2, (size_t)P_OUT * H}, {b.db2, (size_t)P_OUT},
+        {b.dWc0, H * Kin}, {b.dbc0, H}, {b.dWc1, H * H}, {b.dbc1, H}, {b.dWc2, 2 * H * H}, {b.dbc2, 2 * H},
+        {b.dSpeech, (size_t)a.B * a.S}, {b.dStyle, (size_t)a.B * a.Z}};
+    for (const auto& z : zero)
+      if (z.p) ZCHECK_CUDA(cudaMemsetAsync(z.p, 0, z.n * sizeof(float), stream));
+    return ZEGGS_OK;
+  }
   DecGeom g = make_geom(a.B, a.H, a.S, a.Z);
   BwdGeom bg = make_bgeom(g);
   DecWs w = make_ws(a.workspace, g, a.T, 1);

@@ -497,20 +497,20 @@ __global__ void dy_scale_bf16_kernel(const float* __restrict__ dY, const float* 
 }
 
 extern "C" size_t zeggs_decoder_packed_bwd_tc_bytes(int H, int S, int Z) {
-  // the BPTT kernel pairs k-blocks (H % 128 == 0)
-  if (H % 128 != 0 || pick_U(H) <= 0 || H > 1024) return 0;
+  // the BPTT kernel pairs k-blocks (H % 128 == 0, part of tc_hidden_ok)
+  if (!tc_hidden_ok(H)) return 0;
   DecGeom g = make_geom(1, H, S, Z);
   BtGeom tg = make_btgeom(g, make_bgeom(g));
-  if ((tg.kbH % 2) != 0) return 0;
   return (size_t)g.G * tg.cta_bytes;
 }
 extern "C" size_t zeggs_decoder_bwd_tc_workspace_bytes(int H, int S, int Z) {
-  if (H % 64 != 0 || pick_U(H) <= 0 || H > 1024) return 0;
+  if (!tc_hidden_ok(H)) return 0;
   return make_btws(nullptr, make_geom(1, H, S, Z)).bytes;
 }
 extern "C" int zeggs_decoder_pack_weights_bwd_tc(const zeggs_decoder_fwd_args* a, void* packed, void* stream_) {
   CtxScope ctx_scope(a ? a->ctx : nullptr);
-  ZCHECK_ARG(a && packed && a->H % 64 == 0 && pick_U(a->H) > 0, "decoder bwd tc pack: bad arguments");
+  ZCHECK_ARG(a && packed, "decoder bwd tc pack: bad arguments");
+  ZCHECK_SUPPORTED(tc_hidden_ok(a->H), "decoder bwd tc pack: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", a->H);
   const float* mfold = decoder_tc_mfold(*a);
   ZCHECK_ARG(mfold != nullptr, "decoder bwd tc pack: the forward pack (zeggs_decoder_pack_weights_tc -> args.packed_tc) must run first");
   DecGeom g = make_geom(a->B, a->H, a->S, a->Z);

@@ -68,6 +68,10 @@ inline int pick_U(int H) {
   return -1;
 }
 
+// hidden sizes the tensor-core recurrence (engine 1: forward and BPTT kernels) covers; every tc size / pack / run entry point
+// applies this one rule (the BPTT kernel pairs 64-wide k-blocks, and below 384 nothing has been validated)
+inline bool tc_hidden_ok(int H) { return H % 128 == 0 && H >= 384 && H <= 1024; }
+
 struct DecGeom {
   int B, H, S, Z, A;   // A = 1134 + S + Z
   int U, G;            // units per CTA, CTAs

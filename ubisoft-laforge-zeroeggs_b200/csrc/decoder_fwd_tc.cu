@@ -628,18 +628,19 @@ __global__ void __launch_bounds__(256) fold_finish_kernel(zeggs_decoder_fwd_args
 
 // ------------------------------------------------------------------ host
 extern "C" size_t zeggs_decoder_packed_tc_bytes(int H, int S, int Z) {
-  if (H % 64 != 0 || pick_U(H) <= 0 || H > 1024) return 0;
+  if (!tc_hidden_ok(H)) return 0;
   DecGeom g = make_geom(1, H, S, Z);
   return make_tcgeom(g).total_bytes;
 }
 extern "C" size_t zeggs_decoder_tc_workspace_bytes(int H, int S, int Z) {
-  if (H % 64 != 0 || pick_U(H) <= 0 || H > 1024) return 0;
+  if (!tc_hidden_ok(H)) return 0;
   DecGeom g = make_geom(1, H, S, Z);
   return make_tcws(nullptr, g).bytes;
 }
 extern "C" int zeggs_decoder_pack_weights_tc(const zeggs_decoder_fwd_args* a, void* packed, void* stream_) {
   CtxScope ctx_scope(a ? a->ctx : nullptr);
-  ZCHECK_ARG(a && packed && a->H % 64 == 0 && pick_U(a->H) > 0 && a->H <= 1024, "decoder tc pack: bad arguments");
+  ZCHECK_ARG(a && packed, "decoder tc pack: bad arguments");
+  ZCHECK_SUPPORTED(tc_hidden_ok(a->H), "decoder tc pack: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", a->H);
   ZCHECK_ARG(a->in_mean && a->in_std && a->out_mean && a->out_std, "decoder tc pack: normalisation statistics missing");
   cudaStream_t stream = (cudaStream_t)stream_;
   ScopedTimer tm_pack("weight_pack", stream);

@@ -108,14 +108,13 @@ _weights_epoch = 0
 # geometry is eligible, fp32 otherwise).  An explicit "tc" request on an ineligible geometry RAISES (it never silently
 # runs the other engine).
 DECODER_ENGINE = __import__("os").environ.get("ZEGGS_DECODER_ENGINE", "fp32")
-TC_MIN_HIDDEN = 288
 
 
 def tc_eligible(H, S, Z):
     """The tensor-core recurrence (forward AND BPTT kernels) covers H % 128 == 0, 384 <= H <= 1024: the library's
     zeggs_decoder_packed_tc_bytes / _bwd_tc_bytes report 0 for anything else."""
     l = _lib.lib()
-    return H >= TC_MIN_HIDDEN and l.zeggs_decoder_packed_tc_bytes(H, S, Z) > 0 and l.zeggs_decoder_packed_bwd_tc_bytes(H, S, Z) > 0
+    return l.zeggs_decoder_packed_tc_bytes(H, S, Z) > 0 and l.zeggs_decoder_packed_bwd_tc_bytes(H, S, Z) > 0
 
 
 def set_decoder_engine(name):
