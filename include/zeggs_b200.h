@@ -327,7 +327,9 @@ typedef struct {
   const float *Y, *root_pos, *root_rot;
   const float *WY, *W_root_pos, *W_root_rot;
   const float* gaze_pos; /* [B,T,3] */
-  const int* parents;    /* int32 [75] */
+  const int* parents;    /* int32 [75]; must be a tree in topological order: parents[0] == -1 and 0 <= parents[i] < i.
+                            Not checked here (it lives on the device): a cycle or an index >= 75 makes the kernels read and
+                            write out of bounds.  zeggs_b200.train.check_parents validates it on the host. */
   const float *mu, *logvar; /* [B,Z] or NULL */
   float* losses;         /* [19] */
   float *dY, *dRootPos, *dRootRot, *dmu, *dlogvar;

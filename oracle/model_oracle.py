@@ -368,6 +368,30 @@ def train_losses(O, W, gaze_pos, parents, dt, mu=None, logvar=None, iteration=0)
     return total / 18.0, L
 
 
+# static weight of each of the 17 terms (train.py:340-395)
+LOSS_WEIGHTS = dict(root_pos=0.1, root_rot=10.0, root_vel=0.1, root_vrt=5.0, lpos=15.0, lrot=15.0, lvel=10.0, lvrt=7.0,
+                    cpos=0.1, crot=3.0, cvel=0.06, cvrt=1.25, ldvl=7.0, ldvt=8.0, cdvl=0.06, cdvt=1.25, gaze=10.0)
+DIFF_TERMS = ("ldvl", "ldvt", "cdvl", "cdvt")
+
+
+def loss_residuals(O, W, gaze_pos, parents, dt):
+    """The unweighted residuals whose absolute means `train_losses` weights, keyed by term name: term k is
+    LOSS_WEIGHTS[k] * mean(|R[k]|).  Every residual is [B, T', ...] with T' = T for the 13 direct terms (root_rot = root
+    matrix, lrot = raw two-axis ltxy, crot = FK matrix) and T' = T - 1 for the four frame-difference terms, whose index t
+    is the difference between frames t + 1 and t.  Works in the dtype of the inputs."""
+    o = _world_space(*O, parents)
+    w = _world_space(*W, parents)
+    O_gaze = quat_inv_mul_vec(O[1], normalize_vec(gaze_pos - O[0]))
+    W_gaze = quat_inv_mul_vec(W[1], normalize_vec(gaze_pos - W[0]))
+    dv = lambda a, b: (a[:, 1:] - a[:, :-1]) / dt - (b[:, 1:] - b[:, :-1]) / dt
+    R = dict(root_pos=O[0] - W[0], root_rot=o["root_mat"] - w["root_mat"], root_vel=o["root_vel"] - w["root_vel"],
+             root_vrt=o["root_vrt"] - w["root_vrt"], lpos=o["lpos"] - w["lpos"], lrot=O[5] - W[5], lvel=o["lvel"] - w["lvel"],
+             lvrt=o["lvrt"] - w["lvrt"], cpos=o["cpos"] - w["cpos"], crot=o["cmat"] - w["cmat"], cvel=o["cvel"] - w["cvel"],
+             cvrt=o["cvrt"] - w["cvrt"], ldvl=dv(o["lpos"], w["lpos"]), ldvt=dv(O[5], W[5]), cdvl=dv(o["cpos"], w["cpos"]),
+             cdvt=dv(o["cmat"], w["cmat"]), gaze=O_gaze - W_gaze)
+    return R
+
+
 # ----------------------------------------------------------------------------- RAdam
 def radam_step(p, g, m, v, step, lr, beta1=0.9, beta2=0.999, eps=1e-5):
     """optimizers.py:31-99, one parameter tensor, weight_decay=0, degenerated_to_sgd=True.

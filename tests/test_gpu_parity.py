@@ -365,34 +365,6 @@ def test_train_step_loss_and_gradients_vs_reference_golden(dev, golden_dir, gemm
     assert not bad, bad
 
 
-def test_loss_kernel_vs_oracle_autograd(dev):
-    from oracle import model_oracle as mo
-    from zeggs_b200 import synth
-    from zeggs_b200.autograd import TrainLossFn
-    from zeggs_b200.train import pack_pose
-    B, T = 5, 33
-    st = synth.load_stats()
-    O = tt(synth.make_pose_windows(B, T, seed=41)); W = tt(synth.make_pose_windows(B, T, seed=42))
-    rs = np.random.RandomState(0)
-    mu = torch.from_numpy(rs.randn(B, 64).astype(np.float32)); lv = torch.from_numpy((rs.randn(B, 64) * 0.3).astype(np.float32))
-    Ot = [O[k].clone().requires_grad_(True) for k in NAMES]
-    mu_o, lv_o = mu.clone().requires_grad_(True), lv.clone().requires_grad_(True)
-    loss_o, L = mo.train_losses(Ot, [W[k] for k in NAMES], W["gaze_pos"], st["parents"], float(st["dt"]), mu_o, lv_o, 9000)
-    g_ref = torch.autograd.grad(loss_o, Ot + [mu_o, lv_o])
-    Og = [O[k].to(dev).requires_grad_(True) for k in NAMES]
-    mu_g, lv_g = mu.to(dev).requires_grad_(True), lv.to(dev).requires_grad_(True)
-    Y = pack_pose(*Og[2:]); WY = pack_pose(*[W[k].to(dev) for k in NAMES[2:]])
-    terms = torch.zeros(19, device=dev)
-    loss_g = TrainLossFn.apply(Y, Og[0], Og[1], WY, W["root_pos"].to(dev), W["root_rot"].to(dev), W["gaze_pos"].to(dev),
-                               torch.as_tensor(st["parents"], dtype=torch.int32, device=dev), float(st["dt"]), mu_g, lv_g,
-                               mo.kl_weight(9000), terms)
-    g_got = torch.autograd.grad(loss_g, Og + [mu_g, lv_g])
-    assert abs(loss_g.item() - loss_o.item()) <= 2e-5 * abs(loss_o.item())
-    for n, a, b in zip(NAMES + ["mu", "logvar"], g_got, g_ref):
-        err, sc = report(f"loss grad {n}", a, b)
-        assert err <= 3e-4 * max(sc, 1e-9), n
-
-
 def test_fused_radam_vs_reference_golden(dev, golden_dir):
     from zeggs_b200.optimizers import RAdam
     g = np.load(os.path.join(golden_dir, "radam.npz"))

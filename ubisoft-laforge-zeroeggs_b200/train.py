@@ -24,6 +24,23 @@ def kl_weight(iteration, center=7500, rate=0.005, threshold=0.2):
     return min(1.0 / (1.0 + math.exp(-rate * (iteration - center))), threshold)
 
 
+def check_parents(parents, nj=75):
+    """The skeleton's parent array (data_definition.json "parents") as int32, or ValueError unless it is a tree the loss kernel can
+    walk: nj entries, parents[0] == -1 and 0 <= parents[i] < i for every other joint (so no cycles and no second root)."""
+    a = np.asarray(parents)
+    if a.shape != (nj,):
+        raise ValueError(f"parents: expected {nj} joints, got shape {a.shape}")
+    if not np.issubdtype(a.dtype, np.integer):
+        raise ValueError(f"parents: expected integer joint indices, got {a.dtype}")
+    if a[0] != -1:
+        raise ValueError(f"parents[0] must be -1 (the root), got {a[0]}")
+    i = np.arange(1, nj)
+    bad = i[(a[1:] < 0) | (a[1:] >= i)]
+    if bad.size:
+        raise ValueError(f"parents[{bad[0]}] = {a[bad[0]]}: every joint's parent must come before it (0 <= parents[i] < i)")
+    return a.astype(np.int32)
+
+
 def pack_pose(root_vel, root_vrt, lpos, ltxy, lvel, lvrt):
     B, T = root_vel.shape[0], root_vel.shape[1]
     return torch.cat([root_vel.reshape(B, T, -1), root_vrt.reshape(B, T, -1), lpos.reshape(B, T, -1),
@@ -41,13 +58,14 @@ class TrainStep:
 
     def __init__(self, speech_encoder, decoder, style_encoder, stats, parents, dt, lr=1e-4, eps=1e-5,
                  world_size=1, process_group=None, use_graph=False):
+        parents = check_parents(parents)          # before anything reaches the device
         self.se, self.dec, self.st = speech_encoder, decoder, style_encoder
         self.dev = next(decoder.parameters()).device
         f = lambda k: torch.as_tensor(stats[k], dtype=torch.float32, device=self.dev)
         self.audio_mean, self.audio_std = f("audio_input_mean"), f("audio_input_std")
         self.in_mean, self.in_std = f("anim_input_mean"), f("anim_input_std")
         self.out_mean, self.out_std = f("anim_output_mean"), f("anim_output_std")
-        self.parents = torch.as_tensor(np.asarray(parents), dtype=torch.int32, device=self.dev)
+        self.parents = torch.as_tensor(parents, device=self.dev)
         self.dt = float(dt)
         params = list(self.se.parameters()) + list(self.dec.parameters()) + \
             (list(self.st.parameters()) if self.st is not None else [])
