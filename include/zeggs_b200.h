@@ -47,9 +47,9 @@ void zeggs_timing_reset(void);
 int zeggs_timing_read(const char* name, double* total_ms, int* count);
 
 /* ------------------------------------------------------------------------------------------------
- * Per-call context of the batched-GEMM front end (caller-owned, plain data; no library globals are needed when it is passed):
- * every args struct below ends in `const zeggs_ctx* ctx`.  NULL selects the process-wide defaults of the legacy setters
- * (zeggs_set_scratch / zeggs_set_gemm_mode / zeggs_set_fast_wgrad), kept for callers of the plain-argument entry points.
+ * Per-call context of the batched-GEMM front end (caller-owned, plain data; the library keeps no GEMM configuration of its own):
+ * every args struct below ends in `const zeggs_ctx* ctx`.  NULL means no scratch: batched products run on the fp32 SIMT kernel,
+ * convolutions take the im2col path, and the tensor-core decoder backward (which needs scratch) returns ZEGGS_ERR_ARG.
  * Two host threads driving two streams with two contexts never share mutable library state.
  */
 typedef struct {
@@ -151,7 +151,7 @@ typedef struct {
   int engine;            /* 0: fp32 SIMT recurrence (parity grade); 1: tensor-core recurrence, bf16 operands / fp32 state (B <= 32) */
   const void* packed_tc; /* engine 1: zeggs_decoder_pack_weights_tc output */
   void* workspace_tc;    /* engine 1: zeggs_decoder_tc_workspace_bytes bytes (bf16 activation images) */
-  const zeggs_ctx* ctx;  /* GEMM context of this call (NULL: process defaults) */
+  const zeggs_ctx* ctx;  /* GEMM context of this call (NULL: no scratch, see zeggs_ctx) */
 } zeggs_decoder_fwd_args;
 
 size_t zeggs_decoder_packed_bytes(int H, int S, int Z);
@@ -164,11 +164,7 @@ size_t zeggs_decoder_tc_workspace_bytes(int H, int S, int Z);
 int zeggs_decoder_pack_weights_tc(const zeggs_decoder_fwd_args* a, void* packed, void* stream);
 /* development aid: device buffer [64][32] of int64 receiving CTA 0's per-step phase timestamps (NULL = off) */
 void zeggs_debug_set_tc_trace(void* device_buffer);
-void zeggs_debug_set_tc_nacc(int n); /* development aid kept for ABI compatibility: one forward recurrence kernel exists, the value is ignored */
 int zeggs_debug_set_tc_gemm_variant(int v);  /* tensor-core GEMM tile variant: -1 automatic (128x256 tiles for one-pass products with N >= 256, fused three-pass), 0 = 128x128 tiles with streamed passes */
-void zeggs_debug_set_loss_impl(int v); /* development aid: 1 = warp-per-frame loss kernels (default), 0 = round-1 thread-per-frame version */
-void zeggs_debug_set_tc_cluster(int n); /* development aid kept for ABI compatibility: the tc recurrences use no clusters, the value is ignored */
-int zeggs_debug_get_tc_cluster(void);   /* cluster size the last tc forward launch used */
 int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* a, void* stream);
 
 /* Backward of zeggs_decoder_window_fwd (the autograd of modules.py:47-162: full BPTT through the GRU stack,
@@ -418,16 +414,8 @@ int zeggs_tc_gemm_bf16(int M, int N, int K, const void* A_hi, const void* A_lo, 
                        const void* B_lo, int ldb, const float* bias, float* C, int ldc, int act, int accumulate,
                        void* stream);
 /* fp32 GEMM front end used by the encoders: mode 0 NT / 1 TN / 2 NN as zeggs_sgemm.  Large products run on the tensor cores
- * with operands split to bf16 (hi, lo) in the caller-provided scratch buffer (zeggs_set_scratch); small ones on the
- * fp32 SIMT kernel.  zeggs_set_gemm_mode: 0 = fp32 SIMT only, 1 = tensor-core split-bf16 x3 (default), 2 = tensor-core bf16. */
-int zeggs_set_scratch(void* device_ptr, size_t bytes);
-int zeggs_set_gemm_mode(int mode);
-/* 1: weight-gradient products of the encoders (contraction over samples/frames) use ONE bf16 pass instead of the split-bf16
- * three -- the accuracy class of the tensor-core recurrence engine's own weight gradients; set by zeggs_b200.ops.set_decoder_engine. */
-int zeggs_set_fast_wgrad(int on);
-int zeggs_gemm_f32(int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb, const float* bias,
-                   float* C, int ldc, int act, int accumulate, void* stream);
-/* same with an explicit context instead of the process defaults */
+ * with operands split to bf16 (hi, lo) in ctx->scratch, as ctx->gemm_mode and ctx->fast_wgrad select (see zeggs_ctx); small
+ * ones, or any product when ctx is NULL or its scratch is too small, on the fp32 SIMT kernel. */
 int zeggs_gemm_f32_ctx(const zeggs_ctx* ctx, int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                        const float* bias, float* C, int ldc, int act, int accumulate, void* stream);
 int zeggs_split_bf16(const float* x, int rows, int cols, int ld_in, void* hi, void* lo, int ld_out, void* stream);

@@ -135,11 +135,7 @@ SYMBOLS = [
     ("zeggs_decoder_tc_workspace_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_decoder_pack_weights_tc", C.c_int, [C.POINTER(DecoderFwdArgs), C.c_void_p, C.c_void_p]),
     ("zeggs_debug_set_tc_trace", None, [C.c_void_p]),
-    ("zeggs_debug_set_tc_nacc", None, [C.c_int]),
     ("zeggs_debug_set_tc_gemm_variant", C.c_int, [C.c_int]),
-    ("zeggs_debug_set_loss_impl", None, [C.c_int]),
-    ("zeggs_debug_set_tc_cluster", None, [C.c_int]),
-    ("zeggs_debug_get_tc_cluster", C.c_int, []),
     ("zeggs_decoder_packed_bwd_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_decoder_pack_weights_bwd", C.c_int, [C.POINTER(DecoderFwdArgs), C.c_void_p, C.c_void_p]),
     ("zeggs_decoder_bwd_workspace_bytes", C.c_size_t, [C.c_int] * 5),
@@ -158,7 +154,6 @@ SYMBOLS = [
     ("zeggs_style_enc_gru_bwd", C.c_int, [C.POINTER(StyleEncGruArgs), C.POINTER(StyleEncGruGrads), C.c_void_p]),
     ("zeggs_loss_workspace_bytes", C.c_size_t, [C.c_int, C.c_int]),
     ("zeggs_loss_fwd_bwd", C.c_int, [C.POINTER(LossArgs), C.c_void_p]),
-    ("zeggs_set_fast_wgrad", C.c_int, [C.c_int]),
     ("zeggs_dropout_mask", C.c_int, [C.c_void_p, C.c_size_t, C.c_float, C.c_ulonglong, C.c_void_p]),
     ("zeggs_dropout_mask_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_float, C.c_void_p, C.c_ulonglong, C.c_void_p]),
     ("zeggs_randn_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_ulonglong, C.c_void_p]),
@@ -168,10 +163,6 @@ SYMBOLS = [
                                C.c_int, C.c_int, C.c_int, C.c_void_p]),
     ("zeggs_tc_gemm_bf16", C.c_int, [C.c_int] * 3 + [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    ("zeggs_set_scratch", C.c_int, [C.c_void_p, C.c_size_t]),
-    ("zeggs_set_gemm_mode", C.c_int, [C.c_int]),
-    ("zeggs_gemm_f32", C.c_int, [C.c_int] * 4 + [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                  C.c_int, C.c_int, C.c_int, C.c_void_p]),
     ("zeggs_gemm_f32_ctx", C.c_int, [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_int, C.c_int, C.c_void_p]),
     ("zeggs_split_bf16", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),

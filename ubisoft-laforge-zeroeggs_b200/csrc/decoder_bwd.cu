@@ -659,7 +659,7 @@ extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const 
       ZCHECK_ARG(!use_tc, "decoder bwd tc: scratch buffer too small for the batched gradient GEMMs (%zu bytes needed)", need + extra);
     }
   } else {
-    ZCHECK_ARG(!use_tc, "decoder bwd tc: needs the tensor-core GEMM front end (zeggs_set_scratch, gemm mode 1 or 2)");
+    ZCHECK_ARG(!use_tc, "decoder bwd tc: needs the tensor-core GEMM front end (a zeggs_ctx with scratch, gemm mode 1 or 2)");
   }
   if (fold) return ZEGGS_OK;                    // the folded path is complete (CellStateEncoder + scatter ran in phase 1)
 #define WG(...) do { if (!tc_done) { rc = wgrad(__VA_ARGS__); if (rc) return rc; } } while (0)

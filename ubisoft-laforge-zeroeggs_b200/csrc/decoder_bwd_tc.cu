@@ -558,7 +558,7 @@ int decoder_bwd_tc_run(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_
   const int H = a.H, ld = round_up(P_OUT, 8);
   const size_t rows = (size_t)a.B * a.T;
   char* p = scratch_base();
-  ZCHECK_ARG(p != nullptr, "decoder bwd tc: scratch buffer missing (zeggs_set_scratch)");
+  ZCHECK_ARG(p != nullptr, "decoder bwd tc: scratch buffer missing (zeggs_ctx.scratch)");
   auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) / 256 * 256; return r; };
   __nv_bfloat16* dys = (__nv_bfloat16*)take(rows * ld * 2);
   __nv_bfloat16* w2t = (__nv_bfloat16*)take((size_t)H * ld * 2);

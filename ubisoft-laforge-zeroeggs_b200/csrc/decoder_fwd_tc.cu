@@ -672,10 +672,6 @@ extern "C" int zeggs_decoder_pack_weights_tc(const zeggs_decoder_fwd_args* a, vo
   return ZEGGS_OK;
 }
 
-// The recurrences launch without thread-block clusters; the cluster-size knob is kept for ABI compatibility.
-extern "C" void zeggs_debug_set_tc_cluster(int) {}
-extern "C" int zeggs_debug_get_tc_cluster() { return 1; }
-
 template <int U>
 static int launch_tc(const zeggs_decoder_fwd_args& a, const DecGeom& g, const TcGeom& tg, const DecWs& w, const TcWs& tw,
                      const uint8_t* packed, cudaStream_t stream) {
@@ -705,8 +701,6 @@ const float* decoder_tc_mfold(const zeggs_decoder_fwd_args& a) {
 }
 
 static long long* g_tc_dbg = nullptr;
-// one forward kernel configuration exists; the development knob is kept for ABI compatibility and ignored
-extern "C" void zeggs_debug_set_tc_nacc(int) {}
 long long* tc_debug_buffer() { return g_tc_dbg; }
 extern "C" void zeggs_debug_set_tc_trace(void* p) { g_tc_dbg = (long long*)p; }
 

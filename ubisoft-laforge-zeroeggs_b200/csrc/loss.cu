@@ -1,200 +1,98 @@
 // Training loss, forward + backward in one call (ZEGGS/train.py:277-421): local->world transforms, two
-// 75-joint FK passes (output and ground truth), 17 weighted L1 means (4 of them on frame-to-frame
+// 75-joint FK passes (output and ground truth, anim/txform.py:10-34), 17 weighted L1 means (4 of them on frame-to-frame
 // differences) + the annealed KL term, /18 -- and the gradient of that scalar w.r.t. the decoder outputs.
-// Layout: every per-frame quantity lives in structure-of-arrays buffers [channel][frame] so that one thread
-// per frame (lanes = consecutive frames) reads and writes fully coalesced; the AoS pose tensors are
-// transposed in and the gradient transposed out by tiled smem transposes.
+// One warp per frame, one tree level at a time; the kernels are described above loss_tree_kernel.
 #include "decoder_common.cuh"
-#include "loss_frame.cuh"
 
 namespace zeggs {
 
-constexpr int N_TERMS = 17;
-// static L1 weight per Q group and the frame-difference weight (0 = none); train.py:340-395
-struct TermMap { int term; float w; int dterm; float dw; int nch; };
-__host__ __device__ inline TermMap term_of_channel(int ch) {
-  TermMap m;
-  if (ch < Q_ROOT_MAT)      { m.term = 0;  m.w = 0.1f;  m.dterm = -1; m.dw = 0.f;   m.nch = 3; }
-  else if (ch < Q_ROOT_VEL) { m.term = 1;  m.w = 10.f;  m.dterm = -1; m.dw = 0.f;   m.nch = 9; }
-  else if (ch < Q_ROOT_VRT) { m.term = 2;  m.w = 0.1f;  m.dterm = -1; m.dw = 0.f;   m.nch = 3; }
-  else if (ch < Q_LPOS)     { m.term = 3;  m.w = 5.f;   m.dterm = -1; m.dw = 0.f;   m.nch = 3; }
-  else if (ch < Q_LTXY)     { m.term = 4;  m.w = 15.f;  m.dterm = 12; m.dw = 7.f;   m.nch = NJ * 3; }
-  else if (ch < Q_LVEL)     { m.term = 5;  m.w = 15.f;  m.dterm = 13; m.dw = 8.f;   m.nch = NJ * 6; }
-  else if (ch < Q_LVRT)     { m.term = 6;  m.w = 10.f;  m.dterm = -1; m.dw = 0.f;   m.nch = NJ * 3; }
-  else if (ch < Q_CPOS)     { m.term = 7;  m.w = 7.f;   m.dterm = -1; m.dw = 0.f;   m.nch = NJ * 3; }
-  else if (ch < Q_CMAT)     { m.term = 8;  m.w = 0.1f;  m.dterm = 14; m.dw = 0.06f; m.nch = NJ * 3; }
-  else if (ch < Q_CVEL)     { m.term = 9;  m.w = 3.f;   m.dterm = 15; m.dw = 1.25f; m.nch = NJ * 9; }
-  else if (ch < Q_CVRT)     { m.term = 10; m.w = 0.06f; m.dterm = -1; m.dw = 0.f;   m.nch = NJ * 3; }
-  else if (ch < Q_GAZE)     { m.term = 11; m.w = 1.25f; m.dterm = -1; m.dw = 0.f;   m.nch = NJ * 3; }
-  else                      { m.term = 16; m.w = 10.f;  m.dterm = -1; m.dw = 0.f;   m.nch = 3; }
-  return m;
+// ------------------------------------------------------------------ per-frame 3x3 / quaternion math and its adjoints
+struct M3 { float m[9]; };   // row-major
+
+__host__ __device__ inline V3 mv(const M3& a, V3 v) {
+  return v3(a.m[0] * v.x + a.m[1] * v.y + a.m[2] * v.z, a.m[3] * v.x + a.m[4] * v.y + a.m[5] * v.z, a.m[6] * v.x + a.m[7] * v.y + a.m[8] * v.z);
 }
-
-// src [rows][cols] row-major -> dst [cols][ld] (and the inverse), 32x32 tiles
-__global__ void transpose_kernel(const float* __restrict__ src, int rows, int cols, int ld_src, float* __restrict__ dst, int ld_dst) {
-  __shared__ float tile[32][33];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += 8) {
-    int r = r0 + i, c = c0 + threadIdx.x;
-    tile[i][threadIdx.x] = (r < rows && c < cols) ? src[(size_t)r * ld_src + c] : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += 8) {
-    int c = c0 + i, r = r0 + threadIdx.x;
-    if (c < cols && r < rows) dst[(size_t)c * ld_dst + r] = tile[threadIdx.x][i];
-  }
+__host__ __device__ inline V3 mtv(const M3& a, V3 v) {   // a^T v
+  return v3(a.m[0] * v.x + a.m[3] * v.y + a.m[6] * v.z, a.m[1] * v.x + a.m[4] * v.y + a.m[7] * v.z, a.m[2] * v.x + a.m[5] * v.y + a.m[8] * v.z);
 }
-
-struct LossDev {
-  int B, T; float dt;
-  const float *Ys[2]; const float *rp[2]; const float *rq[2];   // [0] = output, [1] = ground truth
-  const float* gaze; const int* parents;
-  float* Q[2]; float* G; float* gYs;
-  size_t stride;
-};
-
-constexpr int LOSS_TB = 64;      // frames per CTA: 8192 frames x 2 sides = 256 CTAs (the per-frame FK chain is latency bound: spread it over every SM)
-
-__global__ void __launch_bounds__(LOSS_TB) loss_fk_fwd_kernel(LossDev d) {
-  __shared__ int s_par[NJ];
-  for (int i = threadIdx.x; i < NJ; i += blockDim.x) s_par[i] = d.parents[i];
-  __syncthreads();
-  const size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  const int X = blockIdx.y;
-  if (idx >= (size_t)d.B * d.T) return;
-  const int t = (int)(idx % d.T);
-  const float* q4 = d.rq[X] + idx * 4;
-  Q4 q; q.w = q4[0]; q.x = q4[1]; q.y = q4[2]; q.z = q4[3];
-  Q4 qp = q;
-  if (t > 0) { qp.w = q4[-4]; qp.x = q4[-3]; qp.y = q4[-2]; qp.z = q4[-1]; }
-  V3 pos = v3(d.rp[X][idx * 3], d.rp[X][idx * 3 + 1], d.rp[X][idx * 3 + 2]);
-  V3 gz = v3(d.gaze[idx * 3], d.gaze[idx * 3 + 1], d.gaze[idx * 3 + 2]);
-  loss_frame_forward(d.Ys[X], d.stride, idx, q, qp, pos, gz, s_par, d.Q[X]);
-}
-
-// one block = 256 consecutive frames of one channel.  partial[(ch*nblk + blk)*2 + {0,1}] = sum |D|, sum |D[t+1]-D[t]|
-__global__ void __launch_bounds__(256) loss_terms_kernel(LossDev d, float* __restrict__ partial, int nblk) {
-  const int ch = blockIdx.y;
-  const size_t idx = blockIdx.x * (size_t)256 + threadIdx.x;
-  const size_t BT = (size_t)d.B * d.T;
-  const TermMap m = term_of_channel(ch);
-  float s0 = 0.f, s1 = 0.f;
-  if (idx < BT) {
-    const int t = (int)(idx % d.T);
-    const float* qo = d.Q[0] + (size_t)ch * d.stride;
-    const float* qw = d.Q[1] + (size_t)ch * d.stride;
-    const float D = qo[idx] - qw[idx];
-    s0 = fabsf(D);
-    const float sg = (D > 0.f) - (D < 0.f);
-    float g = m.w * sg / ((float)BT * (float)m.nch);
-    if (m.dterm >= 0 && d.T > 1) {
-      const float inv_dt = 1.0f / d.dt;
-      const float nd = (float)d.B * (float)(d.T - 1) * (float)m.nch;
-      float gd = 0.f;
-      if (t + 1 < d.T) {   // this frame is the left end of difference t
-        const float e = ((qo[idx + 1] - qo[idx]) * inv_dt) - ((qw[idx + 1] - qw[idx]) * inv_dt);   // train.py:356-393
-        s1 = fabsf(e);
-        gd -= (float)((e > 0.f) - (e < 0.f));
-      }
-      if (t > 0) {
-        const float e = ((qo[idx] - qo[idx - 1]) * inv_dt) - ((qw[idx] - qw[idx - 1]) * inv_dt);
-        gd += (float)((e > 0.f) - (e < 0.f));
-      }
-      g += m.dw * inv_dt * gd / nd;
-    }
-    d.G[(size_t)ch * d.stride + idx] = g * (1.0f / 18.0f);
-  }
-  __shared__ float r0[8], r1[8];
+__host__ __device__ inline M3 mm(const M3& a, const M3& b) {
+  M3 r;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { s0 += __shfl_xor_sync(0xffffffffu, s0, o); s1 += __shfl_xor_sync(0xffffffffu, s1, o); }
-  if ((threadIdx.x & 31) == 0) { r0[threadIdx.x >> 5] = s0; r1[threadIdx.x >> 5] = s1; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float a = 0.f, b = 0.f;
-    for (int i = 0; i < 8; ++i) { a += r0[i]; b += r1[i]; }
-    partial[((size_t)ch * nblk + blockIdx.x) * 2] = a;
-    partial[((size_t)ch * nblk + blockIdx.x) * 2 + 1] = b;
-  }
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) r.m[i * 3 + j] = a.m[i * 3] * b.m[j] + a.m[i * 3 + 1] * b.m[3 + j] + a.m[i * 3 + 2] * b.m[6 + j];
+  return r;
 }
-
-// deterministic reduction, stage 1: one warp per channel sums that channel's per-CTA partials in a fixed order
-// chan[ch][0] = sum |D|, chan[ch][1] = sum |D[t+1] - D[t]| / dt
-__global__ void __launch_bounds__(256) loss_chan_kernel(const float* __restrict__ partial, int nblk, double* __restrict__ chan) {
-  const int ch = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (ch >= Q_CH) return;
-  double l0 = 0.0, l1 = 0.0;
-  for (int i = lane; i < nblk; i += 32) { l0 += partial[((size_t)ch * nblk + i) * 2]; l1 += partial[((size_t)ch * nblk + i) * 2 + 1]; }
-  for (int o = 16; o > 0; o >>= 1) { l0 += __shfl_xor_sync(0xffffffffu, l0, o); l1 += __shfl_xor_sync(0xffffffffu, l1, o); }
-  if (lane == 0) { chan[2 * ch] = l0; chan[2 * ch + 1] = l1; }
+__host__ __device__ inline M3 mtm(const M3& a, const M3& b) {  // a^T b
+  M3 r;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) r.m[i * 3 + j] = a.m[i] * b.m[j] + a.m[3 + i] * b.m[3 + j] + a.m[6 + i] * b.m[6 + j];
+  return r;
 }
-
-// stage 2 + KL (modules.py:764-789).  losses[0] = total, [1..17] = the 17 terms, [18] = kl term
-__global__ void __launch_bounds__(1024) loss_final_kernel(const double* __restrict__ chan, int B, int T, float dt,
-                                                          const float* __restrict__ mu, const float* __restrict__ logvar, int Z,
-                                                          float kl_weight_host, const float* __restrict__ kl_weight_dev,
-                                                          float* __restrict__ losses, float* __restrict__ dmu,
-                                                          float* __restrict__ dlogvar) {
-  // the annealed KL weight (modules.py:745-761) either by value or from device memory (CUDA-graph replays: the host updates
-  // the scalar between replays without re-capturing)
-  const float kl_weight = kl_weight_dev ? *kl_weight_dev : kl_weight_host;
-  __shared__ double wacc[32][N_TERMS + 1];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane <= N_TERMS) wacc[warp][lane] = 0.0;
-  __syncwarp();
-  const double BT = (double)B * T;
-  // warp w owns channels ch = w, w+32, ...: fixed summation order -> bitwise reproducible
-  if (lane == 0) {
-    for (int ch = warp; ch < Q_CH; ch += 32) {
-      const TermMap m = term_of_channel(ch);
-      wacc[warp][m.term] += chan[2 * ch] * ((double)m.w / (BT * m.nch));
-      if (m.dterm >= 0 && T > 1) wacc[warp][m.dterm] += chan[2 * ch + 1] * ((double)m.dw / ((double)B * (T - 1) * m.nch));
-    }
-  }
-  double kl = 0.0;
-  if (mu && logvar) {
-    for (int i = threadIdx.x; i < B * Z; i += blockDim.x) {
-      float m_ = mu[i], lv = logvar[i];
-      kl += -0.5 * (1.0 + lv - (double)m_ * m_ - exp((double)lv));
-      const float gscale = kl_weight / ((float)B * (float)Z) / 18.0f;
-      if (dmu) dmu[i] = gscale * m_;
-      if (dlogvar) dlogvar[i] = gscale * 0.5f * (expf(lv) - 1.0f);
-    }
-  }
-  for (int o = 16; o > 0; o >>= 1) kl += __shfl_xor_sync(0xffffffffu, kl, o);
-  if (lane == 0) wacc[warp][N_TERMS] = kl;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double total = 0.0;
-    for (int term = 0; term <= N_TERMS; ++term) {
-      double s = 0.0;
-      for (int w = 0; w < 32; ++w) s += wacc[w][term];
-      if (term == N_TERMS) s = (mu && logvar) ? kl_weight * s / ((double)B * Z) : 0.0;
-      losses[1 + term] = (float)s;
-      total += s;
-    }
-    losses[0] = (float)(total / 18.0);
-  }
+__host__ __device__ inline M3 mmt(const M3& a, const M3& b) {  // a b^T
+  M3 r;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) r.m[i * 3 + j] = a.m[i * 3] * b.m[j * 3] + a.m[i * 3 + 1] * b.m[j * 3 + 1] + a.m[i * 3 + 2] * b.m[j * 3 + 2];
+  return r;
 }
-
-__global__ void __launch_bounds__(LOSS_TB) loss_fk_bwd_kernel(LossDev d, float* __restrict__ dRootPos, float* __restrict__ dq_own, float* __restrict__ dq_prev) {
-  __shared__ int s_par[NJ];
-  for (int i = threadIdx.x; i < NJ; i += blockDim.x) s_par[i] = d.parents[i];
-  __syncthreads();
-  const size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (idx >= (size_t)d.B * d.T) return;
-  const int t = (int)(idx % d.T);
-  const float* q4 = d.rq[0] + idx * 4;
-  Q4 q; q.w = q4[0]; q.x = q4[1]; q.y = q4[2]; q.z = q4[3];
-  Q4 qp = q;
-  if (t > 0) { qp.w = q4[-4]; qp.x = q4[-3]; qp.y = q4[-2]; qp.z = q4[-1]; }
-  V3 pos = v3(d.rp[0][idx * 3], d.rp[0][idx * 3 + 1], d.rp[0][idx * 3 + 2]);
-  V3 gz = v3(d.gaze[idx * 3], d.gaze[idx * 3 + 1], d.gaze[idx * 3 + 2]);
-  V3 dpos; Q4 dq, dqp;
-  loss_frame_backward(d.Ys[0], d.Q[0], d.G, d.stride, idx, q, qp, pos, gz, s_par, d.gYs, &dpos, &dq, &dqp);
-  if (t == 0) { dq.w += dqp.w; dq.x += dqp.x; dq.y += dqp.y; dq.z += dqp.z; dqp.w = dqp.x = dqp.y = dqp.z = 0.f; }
-  dRootPos[idx * 3] = dpos.x; dRootPos[idx * 3 + 1] = dpos.y; dRootPos[idx * 3 + 2] = dpos.z;
-  dq_own[idx * 4] = dq.w; dq_own[idx * 4 + 1] = dq.x; dq_own[idx * 4 + 2] = dq.y; dq_own[idx * 4 + 3] = dq.z;
-  dq_prev[idx * 4] = dqp.w; dq_prev[idx * 4 + 1] = dqp.x; dq_prev[idx * 4 + 2] = dqp.y; dq_prev[idx * 4 + 3] = dqp.z;
+__host__ __device__ inline void add_outer(M3& d, V3 a, V3 b) {   // d += a b^T
+  d.m[0] += a.x * b.x; d.m[1] += a.x * b.y; d.m[2] += a.x * b.z;
+  d.m[3] += a.y * b.x; d.m[4] += a.y * b.y; d.m[5] += a.y * b.z;
+  d.m[6] += a.z * b.x; d.m[7] += a.z * b.y; d.m[8] += a.z * b.z;
+}
+__host__ __device__ inline M3 quat_to_xform(Q4 q) {  // tquat.py:53-67
+  float x2 = q.x + q.x, y2 = q.y + q.y, z2 = q.z + q.z;
+  float xx = q.x * x2, yy = q.y * y2, wx = q.w * x2;
+  float xy = q.x * y2, yz = q.y * z2, wy = q.w * y2;
+  float xz = q.x * z2, zz = q.z * z2, wz = q.w * z2;
+  M3 r;
+  r.m[0] = 1.0f - (yy + zz); r.m[1] = xy - wz; r.m[2] = xz + wy;
+  r.m[3] = xy + wz; r.m[4] = 1.0f - (xx + zz); r.m[5] = yz - wx;
+  r.m[6] = xz - wy; r.m[7] = yz + wx; r.m[8] = 1.0f - (xx + yy);
+  return r;
+}
+__host__ __device__ inline Q4 quat_to_xform_bwd(Q4 q, const M3& d) {
+  Q4 g;
+  g.w = 2.0f * (-q.z * d.m[1] + q.y * d.m[2] + q.z * d.m[3] - q.x * d.m[5] - q.y * d.m[6] + q.x * d.m[7]);
+  g.x = 2.0f * (q.y * d.m[1] + q.z * d.m[2] + q.y * d.m[3] - 2.0f * q.x * d.m[4] - q.w * d.m[5] + q.z * d.m[6] + q.w * d.m[7] - 2.0f * q.x * d.m[8]);
+  g.y = 2.0f * (-2.0f * q.y * d.m[0] + q.x * d.m[1] + q.w * d.m[2] + q.x * d.m[3] + q.z * d.m[5] - q.w * d.m[6] + q.z * d.m[7] - 2.0f * q.y * d.m[8]);
+  g.z = 2.0f * (-2.0f * q.z * d.m[0] - q.w * d.m[1] + q.x * d.m[2] + q.w * d.m[3] - 2.0f * q.z * d.m[4] + q.y * d.m[5] + q.x * d.m[6] + q.y * d.m[7]);
+  return g;
+}
+// u = v / (|v| + eps) and its adjoint
+__host__ __device__ inline V3 unit_eps(V3 v, float eps) { float n = sqrtf(dot(v, v)); return (1.0f / (n + eps)) * v; }
+__host__ __device__ inline V3 unit_eps_bwd(V3 v, float eps, V3 du) {
+  float n = sqrtf(dot(v, v));
+  V3 r = (1.0f / (n + eps)) * du;
+  if (n > 0.0f) r = r - (dot(du, v) / ((n + eps) * (n + eps) * n)) * v;
+  return r;
+}
+// txform.py:23-34: columns of the result are the normalised x, y = z cross x, z = x cross xy[1] axes
+__host__ __device__ inline M3 orthogonalize_xy(V3 x, V3 yv) {
+  V3 z = cross(x, yv), y = cross(z, x);
+  V3 X = unit_eps(x, 1e-10f), Y = unit_eps(y, 1e-10f), Z = unit_eps(z, 1e-10f);
+  M3 r;
+  r.m[0] = X.x; r.m[1] = Y.x; r.m[2] = Z.x;
+  r.m[3] = X.y; r.m[4] = Y.y; r.m[5] = Z.y;
+  r.m[6] = X.z; r.m[7] = Y.z; r.m[8] = Z.z;
+  return r;
+}
+__host__ __device__ inline void orthogonalize_xy_bwd(V3 x, V3 yv, const M3& d, V3& dx, V3& dyv) {
+  V3 z = cross(x, yv), y = cross(z, x);
+  V3 dX = v3(d.m[0], d.m[3], d.m[6]), dY = v3(d.m[1], d.m[4], d.m[7]), dZ = v3(d.m[2], d.m[5], d.m[8]);
+  dx = unit_eps_bwd(x, 1e-10f, dX);
+  V3 dy = unit_eps_bwd(y, 1e-10f, dY);
+  V3 dz = unit_eps_bwd(z, 1e-10f, dZ);
+  // y = z x x
+  dz = dz + cross(x, dy);
+  dx = dx + cross(dy, z);
+  // z = x x yv
+  dx = dx + cross(yv, dz);
+  dyv = cross(dz, x);
 }
 
 // dRootRot[b][t] = own[b][t] + prev[b][t+1]
@@ -206,17 +104,18 @@ __global__ void root_rot_combine_kernel(const float* __restrict__ own, const flo
 }
 
 // ================================================================================================================
-// Warp-per-frame implementation (round 2; zeggs_loss_fwd_bwd's default).  One warp owns one frame; the joints of one tree level are
-// processed in parallel (the shipped skeleton: 13 levels, at most 12 joints wide), every world-space quantity lives in shared
-// memory, and the only global intermediates are the differences D of the four channel groups whose frame-to-frame terms need the
-// neighbouring frames (1575 floats per frame) plus 17 per-frame partial sums.  The large structure-of-arrays buffers of the
-// thread-per-frame version (74-deep dependent chains through L2) are gone; results are bitwise reproducible (fixed shuffle and frame
+// One warp owns one frame; the joints of one tree level are processed in parallel (the shipped skeleton: 13 levels, at most 12
+// joints wide) and every world-space quantity lives in shared memory.  The only global intermediates are the differences D of the
+// four channel groups whose frame-to-frame terms need the neighbouring frames (1575 floats per frame), 17 per-frame partial sums,
+// the signs of D and the output-side FK results the adjoint re-reads.  Results are bitwise reproducible (fixed shuffle and frame
 // orders).
+//   K0 loss_tree_kernel    level order and child lists of the skeleton, from `parents`
 //   K1 loss_w_fwd_kernel   FK of the output (lanes 0..15) and of the target (lanes 16..31), D, direct |D| sums, D rows of the diff groups
 //                          + the signs of D (2 x 33 bits per joint) and the output-side FK rotations / angular velocities for K2
 //   K2 loss_w_bwd_kernel   two frames per warp, no forward recompute: builds dLoss/dQ from K1's signs (direct terms) and the
 //                          neighbours' D rows (frame-difference terms), runs the adjoint FK level by level (children publish their
 //                          contribution, parents gather them in index order), writes the dY row + the root gradients
+//                          (forward-only calls run loss_w_diff_kernel instead: the frame-difference sums alone)
 //   K3 loss_w_final_kernel deterministic reduction over frames + KL
 // The frame-difference residual is evaluated as (D[t+1] - D[t]) / dt with D = Q_out - Q_target (train.py:356-393 computes
 // dQ_out/dt - dQ_target/dt: equal up to fp32 rounding).
@@ -281,8 +180,8 @@ constexpr int LW_Q = NJ * LW_REC;                // 2475 floats per side
 constexpr int LW_RT = 24;                        // root block: pos3 R9 velw3 vrtw3 gaze3
 constexpr int LW_DD = NJ * 21;                   // 1575: D rows of LPOS (225) | LTXY (450) | CPOS (225) | CMAT (675)
 constexpr int LW_FWD_FLOATS = 2 * LW_Q + 2 * LW_RT;
-constexpr int LW_NP = 17;
-constexpr int LW_SW = NJ * 4 + 2;                // sign words per frame: joint i -> pos_lo, pos_hi, neg_lo, neg_hi (33 bits each); root pos, neg                        // partial sums per frame: terms 0..11, gaze, then the 4 frame-difference terms
+constexpr int LW_NP = 17;                        // partial sums per frame: terms 0..11, gaze, then the 4 frame-difference terms
+constexpr int LW_SW = NJ * 4 + 2;                // sign words per frame: joint i -> pos_lo, pos_hi, neg_lo, neg_hi (33 bits each); root pos, neg
 
 struct LossWArgs {
   int B, T; float dt;
@@ -683,27 +582,16 @@ __global__ void __launch_bounds__(LW_NP * 32) loss_w_final_kernel(const float* _
   }
 }
 
-struct LossWs { float *Ys[2], *Q[2], *G, *gYs, *partial, *dq_own, *dq_prev; double* chan; float* Dd; float* fpartial; TreeTables* tt; float* F; unsigned* S; size_t stride; int nblk; size_t bytes; };
+struct LossWs { float *Dd, *fpartial, *F, *dq_own, *dq_prev; unsigned* S; TreeTables* tt; size_t bytes; };
 static LossWs loss_ws(void* base, int B, int T) {
   LossWs w; size_t off = 0;
   auto take = [&](size_t n) { float* p = base ? (float*)((char*)base + off) : nullptr; off += ((n * 4 + 255) / 256) * 256; return p; };
   const size_t BT = (size_t)B * T;
-  w.stride = (BT + 31) / 32 * 32;
-  w.nblk = (int)((BT + 255) / 256);
-  for (int x = 0; x < 2; ++x) w.Ys[x] = take((size_t)P_OUT * w.stride);
-  for (int x = 0; x < 2; ++x) w.Q[x] = take((size_t)Q_CH * w.stride);
-  w.G = take((size_t)Q_CH * w.stride);
-  w.gYs = take((size_t)P_OUT * w.stride);
-  w.partial = take((size_t)Q_CH * w.nblk * 2);
   w.dq_own = take(BT * 4); w.dq_prev = take(BT * 4);
-  w.chan = (double*)take((size_t)Q_CH * 4);
   w.Dd = take(BT * LW_DD); w.fpartial = take(BT * LW_NP); w.tt = (TreeTables*)take(sizeof(TreeTables) / 4 + 1);
   w.F = take(BT * NJ * 12); w.S = (unsigned*)take(BT * LW_SW);
   w.bytes = off; return w;
 }
-// 1: warp-per-frame kernels (default), 0: the thread-per-frame SoA version of round 1 (kept as a cross-check)
-static int g_loss_impl = 1;
-extern "C" void zeggs_debug_set_loss_impl(int v) { g_loss_impl = v ? 1 : 0; }
 extern "C" size_t zeggs_loss_workspace_bytes(int B, int T) { return (B < 1 || T < 1) ? 0 : loss_ws(nullptr, B, T).bytes; }
 
 extern "C" int zeggs_loss_fwd_bwd(const zeggs_loss_args* ap, void* stream_) {
@@ -716,53 +604,31 @@ extern "C" int zeggs_loss_fwd_bwd(const zeggs_loss_args* ap, void* stream_) {
   const int BT = a.B * a.T;
   ZCHECK_ARG((long long)a.B * a.T < (1ll << 31), "loss: too many frames");
   ScopedTimer tm("loss", s);
-  if (g_loss_impl == 1) {
-    LossWArgs wa;
-    wa.B = a.B; wa.T = a.T; wa.dt = a.dt;
-    wa.Y[0] = a.Y; wa.Y[1] = a.WY; wa.rp[0] = a.root_pos; wa.rp[1] = a.W_root_pos; wa.rq[0] = a.root_rot; wa.rq[1] = a.W_root_rot;
-    wa.gaze = a.gaze_pos; wa.tt = w.tt; wa.Dd = w.Dd; wa.partial = w.fpartial; wa.F = w.F; wa.S = w.S;
-    wa.dY = a.dY; wa.dRootPos = a.dRootPos; wa.dq_own = w.dq_own; wa.dq_prev = w.dq_prev;
-    static bool attr = false;
-    if (!attr) {
-      ZCHECK_CUDA(cudaFuncSetAttribute(loss_w_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LW_WARPS * LW_FWD_FLOATS * sizeof(float))));
-      ZCHECK_CUDA(cudaFuncSetAttribute(loss_w_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LB_WARPS * 2 * LB_FRAME_FLOATS * sizeof(float))));
-      attr = true;
-    }
-    loss_tree_kernel<<<1, 96, 0, s>>>(a.parents, w.tt); count_launch();
-    const int nb = ceil_div(BT, LW_WARPS);
-    loss_w_fwd_kernel<<<nb, LW_WARPS * 32, LW_WARPS * LW_FWD_FLOATS * sizeof(float), s>>>(wa); count_launch();
-    if (a.dY) {
-      ZCHECK_ARG(a.dRootPos && a.dRootRot, "loss: gradient outputs missing");
-      loss_w_bwd_kernel<<<ceil_div(BT, LB_WARPS * 2), LB_WARPS * 32, LB_WARPS * 2 * LB_FRAME_FLOATS * sizeof(float), s>>>(wa); count_launch();
-      root_rot_combine_kernel<<<ceil_div(BT * 4, 256), 256, 0, s>>>(w.dq_own, w.dq_prev, a.B, a.T, a.dRootRot); count_launch();
-    } else if (a.T > 1) {
-      wa.dY = nullptr;
-      loss_w_diff_kernel<<<ceil_div(BT, 8), 256, 0, s>>>(wa); count_launch();
-    }
-    loss_w_final_kernel<<<1, LW_NP * 32, 0, s>>>(w.fpartial, a.B, a.T, a.mu, a.logvar, a.Z, a.kl_weight, a.kl_weight_dev, a.losses, a.dmu, a.dlogvar);
-    count_launch();
-    ZCHECK_LAUNCH();
-    return ZEGGS_OK;
+  LossWArgs wa;
+  wa.B = a.B; wa.T = a.T; wa.dt = a.dt;
+  wa.Y[0] = a.Y; wa.Y[1] = a.WY; wa.rp[0] = a.root_pos; wa.rp[1] = a.W_root_pos; wa.rq[0] = a.root_rot; wa.rq[1] = a.W_root_rot;
+  wa.gaze = a.gaze_pos; wa.tt = w.tt; wa.Dd = w.Dd; wa.partial = w.fpartial; wa.F = w.F; wa.S = w.S;
+  wa.dY = a.dY; wa.dRootPos = a.dRootPos; wa.dq_own = w.dq_own; wa.dq_prev = w.dq_prev;
+  static bool attr = false;
+  if (!attr) {
+    ZCHECK_CUDA(cudaFuncSetAttribute(loss_w_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LW_WARPS * LW_FWD_FLOATS * sizeof(float))));
+    ZCHECK_CUDA(cudaFuncSetAttribute(loss_w_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LB_WARPS * 2 * LB_FRAME_FLOATS * sizeof(float))));
+    attr = true;
   }
-  dim3 tb(32, 8);
-  transpose_kernel<<<dim3(ceil_div(P_OUT, 32), ceil_div(BT, 32)), tb, 0, s>>>(a.Y, BT, P_OUT, P_OUT, w.Ys[0], (int)w.stride); count_launch();
-  transpose_kernel<<<dim3(ceil_div(P_OUT, 32), ceil_div(BT, 32)), tb, 0, s>>>(a.WY, BT, P_OUT, P_OUT, w.Ys[1], (int)w.stride); count_launch();
-  LossDev d;
-  d.B = a.B; d.T = a.T; d.dt = a.dt;
-  d.Ys[0] = w.Ys[0]; d.Ys[1] = w.Ys[1]; d.rp[0] = a.root_pos; d.rp[1] = a.W_root_pos; d.rq[0] = a.root_rot; d.rq[1] = a.W_root_rot;
-  d.gaze = a.gaze_pos; d.parents = a.parents; d.Q[0] = w.Q[0]; d.Q[1] = w.Q[1]; d.G = w.G; d.gYs = w.gYs; d.stride = w.stride;
-  loss_fk_fwd_kernel<<<dim3(ceil_div(BT, LOSS_TB), 2), LOSS_TB, 0, s>>>(d); count_launch();
-  loss_terms_kernel<<<dim3(w.nblk, Q_CH), 256, 0, s>>>(d, w.partial, w.nblk); count_launch();
-  loss_chan_kernel<<<ceil_div(Q_CH, 8), 256, 0, s>>>(w.partial, w.nblk, w.chan); count_launch();
-  loss_final_kernel<<<1, 1024, 0, s>>>(w.chan, a.B, a.T, a.dt, a.mu, a.logvar, a.Z, a.kl_weight, a.kl_weight_dev, a.losses, a.dmu, a.dlogvar); count_launch();
-  ZCHECK_LAUNCH();
+  loss_tree_kernel<<<1, 96, 0, s>>>(a.parents, w.tt); count_launch();
+  const int nb = ceil_div(BT, LW_WARPS);
+  loss_w_fwd_kernel<<<nb, LW_WARPS * 32, LW_WARPS * LW_FWD_FLOATS * sizeof(float), s>>>(wa); count_launch();
   if (a.dY) {
     ZCHECK_ARG(a.dRootPos && a.dRootRot, "loss: gradient outputs missing");
-    loss_fk_bwd_kernel<<<ceil_div(BT, LOSS_TB), LOSS_TB, 0, s>>>(d, a.dRootPos, w.dq_own, w.dq_prev); count_launch();
+    loss_w_bwd_kernel<<<ceil_div(BT, LB_WARPS * 2), LB_WARPS * 32, LB_WARPS * 2 * LB_FRAME_FLOATS * sizeof(float), s>>>(wa); count_launch();
     root_rot_combine_kernel<<<ceil_div(BT * 4, 256), 256, 0, s>>>(w.dq_own, w.dq_prev, a.B, a.T, a.dRootRot); count_launch();
-    transpose_kernel<<<dim3(ceil_div(BT, 32), ceil_div(P_OUT, 32)), tb, 0, s>>>(w.gYs, P_OUT, BT, (int)w.stride, a.dY, P_OUT); count_launch();
-    ZCHECK_LAUNCH();
+  } else if (a.T > 1) {
+    wa.dY = nullptr;
+    loss_w_diff_kernel<<<ceil_div(BT, 8), 256, 0, s>>>(wa); count_launch();
   }
+  loss_w_final_kernel<<<1, LW_NP * 32, 0, s>>>(w.fpartial, a.B, a.T, a.mu, a.logvar, a.Z, a.kl_weight, a.kl_weight_dev, a.losses, a.dmu, a.dlogvar);
+  count_launch();
+  ZCHECK_LAUNCH();
   return ZEGGS_OK;
 }
 

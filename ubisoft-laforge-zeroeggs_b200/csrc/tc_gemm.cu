@@ -415,29 +415,18 @@ int split_t_launch(const float* x, int rows, int cols, int ld_in, __nv_bfloat16*
 }
 
 // ------------------------------------------------------------------ fp32-in / fp32-out front end
-// Caller-provided scratch for the bf16 operand copies (the library allocates nothing itself).
-static char* g_scratch = nullptr;
-static size_t g_scratch_bytes = 0;
-static int g_gemm_mode = 1;   // 0: fp32 SIMT everywhere, 1: tensor-core split-bf16 (x3, ~fp32 accuracy), 2: tensor-core plain bf16
-static int g_fast_wgrad = 0;  // 1: weight-gradient products (mode 1, contraction over samples/frames) run as ONE bf16 pass -- set together
-                              //    with the tensor-core recurrence engine, whose own weight gradients are single-pass bf16 already
-
-extern "C" int zeggs_set_scratch(void* p, size_t bytes) { g_scratch = (char*)p; g_scratch_bytes = bytes; return ZEGGS_OK; }
-extern "C" int zeggs_set_gemm_mode(int mode) {
-  ZCHECK_ARG(mode >= 0 && mode <= 2, "gemm mode must be 0 (fp32 SIMT), 1 (tensor-core bf16x3) or 2 (tensor-core bf16)");
-  g_gemm_mode = mode; return ZEGGS_OK;
-}
-extern "C" int zeggs_set_fast_wgrad(int on) { g_fast_wgrad = on ? 1 : 0; return ZEGGS_OK; }
 // The context of the entry point currently executing on this host thread (CtxScope in decoder_common.cuh): per-call state passed
-// by the caller; the process-wide values above are only the defaults for calls that pass none.
-static thread_local const zeggs_ctx* tl_ctx = nullptr;
+// by the caller.  Calls that pass none get k_no_ctx: no scratch, so products run on the fp32 SIMT kernel and convolutions take the
+// im2col path.
+static const zeggs_ctx k_no_ctx = {nullptr, 0, 1, 0};
+static thread_local const zeggs_ctx* tl_ctx = &k_no_ctx;
 static thread_local int tl_fast_wgrad_override = -1;
 const zeggs_ctx* swap_ctx(const zeggs_ctx* c) { const zeggs_ctx* old = tl_ctx; tl_ctx = c; return old; }
-static int fast_wgrad() { return tl_fast_wgrad_override >= 0 ? tl_fast_wgrad_override : (tl_ctx ? tl_ctx->fast_wgrad : g_fast_wgrad); }
+static int fast_wgrad() { return tl_fast_wgrad_override >= 0 ? tl_fast_wgrad_override : tl_ctx->fast_wgrad; }
 int set_fast_wgrad_internal(int on) { const int old = tl_fast_wgrad_override; tl_fast_wgrad_override = on; return old; }
-int gemm_mode() { return tl_ctx ? tl_ctx->gemm_mode : g_gemm_mode; }
-char* scratch_base() { return tl_ctx ? (char*)tl_ctx->scratch : g_scratch; }
-size_t scratch_bytes() { return tl_ctx ? tl_ctx->scratch_bytes : g_scratch_bytes; }
+int gemm_mode() { return tl_ctx->gemm_mode; }
+char* scratch_base() { return (char*)tl_ctx->scratch; }
+size_t scratch_bytes() { return tl_ctx->scratch_bytes; }
 
 int split_hist_launch(const float* x, long long slot_stride, int S, int R, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t stream,
                       float* rowsum, int s_begin) {
@@ -605,10 +594,6 @@ int conv_gemm_wgrad(const float* dpre, int N, const float* x, int B, int T, int 
   return tc_gemm_launch(N, K, M, Ah, Al, Mp, Bh, Bl, Mp, nullptr, dW, K, 0, 0, stream, (float*)p, (size_t)(sbase + sbytes - p));
 }
 
-extern "C" int zeggs_gemm_f32(int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb, const float* bias,
-                              float* C, int ldc, int act, int accumulate, void* stream) {
-  return gemm_f32_auto(mode, M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, (cudaStream_t)stream);
-}
 extern "C" int zeggs_gemm_f32_ctx(const zeggs_ctx* ctx, int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                                   const float* bias, float* C, int ldc, int act, int accumulate, void* stream) {
   CtxScope scope(ctx);
