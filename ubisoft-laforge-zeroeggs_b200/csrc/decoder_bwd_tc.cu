@@ -2,12 +2,18 @@
 // between stages, every transposed GEMM a wgmma chain.
 //
 // The gradient w.r.t. a GRU layer's gate pre-activations is four H-vectors per sample: dpr, dpz, dpn (= d gi) and
-// dpn*r (the n-block of d gh).  They are stored as ONE bf16 image of 128 rows = 4 blocks x 32 samples, K = H, so
-// the 128 rows of two m64 MMAs are fully used and the K = 3H contractions of the SIMT formulation
-// (dh_below = W_ih^T dgi, dh_prev = W_hh^T dgh) collapse into a single K = H chain per layer:
+// dpn*r (the n-block of d gh).  They are stored as ONE bf16 image of 128 rows = 4 blocks x 32 samples in the order
+// [pr, pnr | pz, pn], K = H, and the K = 3H contractions of the SIMT formulation (dh_below = W_ih^T dgi,
+// dh_prev = W_hh^T dgh) collapse into a single K = H chain per layer:
 //     D[(blk,b)][(w,j)] = sum_k img[(blk,b)][k] * Wt[(w,j)][k]
-// and the wanted sums are the block-diagonal entries (pr with *_r, pz with *_z, pn with ih_n, pnr with hh_n), added
-// up by the epilogue from the accumulator staged in shared memory.
+// of which only the block-diagonal entries are wanted (pr with *_r, pz with *_z, pn with ih_n, pnr with hh_n).
+//
+// The grid runs as clusters of 2 CTAs.  A pair covers the 2U units of CTAs 2p and 2p+1 and splits the image by row
+// halves: rank 0 streams rows 0..63 (pr, pnr) of every k-block tile and multiplies them by the columns they pair with
+// (ih_r, hh_r, hh_n), rank 1 streams rows 64..127 (pz, pn) against (ih_z, hh_z, ih_n), each over the full K in one
+// m64 accumulator.  So each SM receives half the image bytes and no MMA is spent on off-diagonal blocks.  Each rank
+// stages its accumulator in its own shared memory, and the epilogue of either rank reads the entries for its own U
+// units from both staging buffers (distributed shared memory), adding them in the same order as a single CTA would.
 //
 // Layer 2 is FOLDED out of the recurrence exactly as in the forward (decoder_fwd_tc.cu): with
 // Mfold = (Wx[:, :1131] diag(os/is)) W2,
@@ -16,8 +22,9 @@
 //              + W2[0:6]^T (os * dch(t-1))                     -- root-integration adjoint, run redundantly by every CTA
 //              + (GRU1 recurrent terms),
 // where the gaze adjoint feeding the root chain needs Wx[:, 1131:1134]^T dS1(t): three more columns per block.
-//   B2  A = G1 image [128 x H],   B = [W_ih1^T | W_hh1^T]                       -> dh0 (+GRU0 adjoint -> G0 image), dh1(t-1) part
-//   B3  A = G0 image [128 x H],   B = [W_ih0a^T | W_hh0^T | 3 x (Mfold_g^T, Wgz_g^T)] -> d pre_a image, dh0(t-1), fold / gaze parts
+//   B2  A = G1 image [64 of 128 x H],  B = 3 of [W_ih1^T | W_hh1^T]             -> dh0 (+GRU0 adjoint -> G0 image), dh1(t-1) part
+//   B3  A = G0 image [64 of 128 x H],  B = 3 of [W_ih0a^T | W_hh0^T], 1 or 2 of 3 x (Mfold_g^T, Wgz_g^T)
+//                                                                                -> d pre_a image, dh0(t-1), fold / gaze parts
 //   B4  A = d pre_a image [32 x H], B = [Mfold_a^T | Wgz_a^T]                  -> fold / gaze parts -> R(t-1): root adjoint,
 //                                                                                  dh1(t-1) -> GRU1 gate adjoint -> G1 image
 // The x_pose / layer-2 gradient history the weight gradients need (DY) is rebuilt after the recurrence by two batched
@@ -29,64 +36,70 @@
 
 namespace zeggs {
 
-constexpr int BT_RING = 3;               // unified operand ring: each slot = 2 k-blocks of (A tile 16 KB | B tile)
-constexpr int BT_XPART = 32768;          // bytes of the A part of a slot
-constexpr int BT_ACC_LD = 132;           // column stride (floats) of the staged accumulator: 128 rows + 4 (bank spread)
+constexpr int BT_RING = 4;               // unified operand ring: each slot = 2 k-blocks of (A half tile 8 KB | B tile)
+constexpr int BT_XPART = 16384;          // bytes of the A part of a slot
+constexpr int BT_ACC_LD = 68;            // column stride (floats) of a staged accumulator: 64 rows + 4 (bank spread)
 
+// Column groups of a pair (2U units: CTA 2p's, then CTA 2p+1's).  B2 / B3 begin with three gate groups of 2U columns:
+// rank 0 (image rows pr, pnr) ih_r, hh_r, hh_n; rank 1 (pz, pn) ih_z, hh_z, ih_n.  B3 then has the fold / gaze groups of the
+// blocks the rank holds (rank 0: gate r; rank 1: gates z, n), FG columns each: 2U Mfold columns and 3 gaze columns, padded.
+// Three fold groups over two ranks make rank 1's B3 chain the wider one (U = 8: 96 vs 72 columns).
 struct BtGeom {
-  int N2, N3, N4, P6;
+  int N2, N3[2], N4, FG;  // chain widths (B3 per cluster rank), fold group width
   int kbH;
   int wslot;              // bytes of one weight k-block tile slot (max N * 128, 1 KB aligned)
   int slot_bytes;         // BT_XPART + 2 * wslot
-  size_t off[4];          // chains: 0 = B2, 1 = B3, 2 = B4
-  size_t cta_bytes;
+  size_t off[3];          // chains: 0 = B2, 1 = B3, 2 = B4; B3 last, so that only the block's length depends on the rank
+  size_t cta_bytes;       // rank 1's block (the longer one); rank 0's ends with unused bytes
 };
 
 inline BtGeom make_btgeom(const DecGeom& g, const BwdGeom&) {
   BtGeom t;
-  t.P6 = round_up(6 * g.U, 16); t.N2 = t.P6; t.N3 = t.P6 + 48; t.N4 = 16;
+  t.FG = round_up(2 * g.U + 3, 8);
+  t.N2 = 6 * g.U; t.N3[0] = t.N2 + t.FG; t.N3[1] = t.N2 + 2 * t.FG; t.N4 = 16;
   t.kbH = ceil_div(g.H, 64);
-  t.wslot = round_up(t.N3 * 128, 1024);
+  t.wslot = round_up(t.N3[1] * 128, 1024);
   t.slot_bytes = BT_XPART + 2 * t.wslot;
-  size_t off = 0;
-  t.off[0] = off; off += (size_t)t.kbH * t.N2 * 128;
-  t.off[1] = off; off += (size_t)t.kbH * t.N3 * 128;
-  t.off[2] = off; off += (size_t)t.kbH * t.N4 * 128;
-  t.off[3] = off;
-  t.cta_bytes = off;
+  t.off[0] = 0;
+  t.off[2] = (size_t)t.kbH * t.N2 * 128;
+  t.off[1] = t.off[2] + (size_t)t.kbH * t.N4 * 128;
+  t.cta_bytes = t.off[1] + (size_t)t.kbH * t.N3[1] * 128;
   return t;
 }
 
-// B3's extra 48 rows = three 16-row groups (gates r, z, n of d gi0): rows 0..U-1 = Mfold[(1+g)H + k][j] (this CTA's units j),
-// rows 8..10 = W_ih0[gH + k][H + 1131 + d] (gaze columns); B4's 16 rows: the same with the pre_a block / W0.
-// One thread per 16-byte image chunk, rows fastest: for a fixed k the 8 units of a row group are contiguous in the source
+// Weight blocks per (pair p, rank rk) with the column groups above.  Gate group columns: unit p*2U + w of W^T for the group's
+// (matrix, gate); fold group of gate gq: columns 0..2U-1 = Mfold[(1+gq)H + k][p*2U + w], 2U..2U+2 = W_ih0[gq H + k][H + 1131 + d]
+// (gaze).  B4 is per CTA: rows 0..U-1 = Mfold[k][j] (this CTA's units j), rows 8..10 = W0[k][1131 + d].
+// One thread per 16-byte image chunk, rows fastest: for a fixed k the units of a column group are contiguous in the source
 // (the weights are read transposed), so a warp reads full 32-byte segments.
 __global__ void pack_decoder_bwd_tc_kernel(DecGeom g, BtGeom tg, const float* __restrict__ Mfold, const float* __restrict__ W0,
                                            const float* __restrict__ Wih0, const float* __restrict__ Whh0,
                                            const float* __restrict__ Wih1, const float* __restrict__ Whh1, uint8_t* __restrict__ out) {
-  const int H = g.H, U = g.U, A = g.A;
+  const int H = g.H, U = g.U, A = g.A, N2 = tg.N2, FG = tg.FG;
   const size_t per = tg.cta_bytes / 16, total = (size_t)g.G * per;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i / per);
+    const int c = (int)(i / per), rk = c & 1, p = c >> 1;
     size_t ci = i % per;                                // chunk index inside the CTA block, re-ordered (kb, logical chunk, row)
-    int chain = 2;
-    for (int q = 0; q < 2; ++q) if (ci < tg.off[q + 1] / 16) { chain = q; break; }
+    const int chain = ci < tg.off[2] / 16 ? 0 : ci < tg.off[1] / 16 ? 2 : 1;
     ci -= tg.off[chain] / 16;
-    const int N = chain == 0 ? tg.N2 : chain == 1 ? tg.N3 : tg.N4;
+    const int N = chain == 0 ? N2 : chain == 1 ? tg.N3[rk] : tg.N4;
+    if (ci >= (size_t)tg.kbH * 8 * N) continue;        // the unused tail of rank 0's block
     const int row = (int)(ci % N), cl = (int)((ci / N) % 8), kb = (int)(ci / ((size_t)8 * N));
     const int k0 = kb * 64 + cl * 8;
     const float* src = nullptr; size_t stride = 0;      // element e of the chunk = src[e * stride]
     if (k0 < H) {
-      if (chain <= 1 && row < 6 * U) {                  // gate-row transposes
-        const int wsel = row / U, u = row % U, gq = wsel % 3, j = c * U + u;
+      if (chain <= 1 && row < N2) {                     // gate-row transposes
+        const int grp = row / (2 * U), j = p * 2 * U + row % (2 * U);
+        const bool ih = rk == 0 ? grp == 0 : grp != 1;
+        const int gq = grp == 2 ? 2 : rk;
         const size_t r = (size_t)(gq * H + k0);
-        if (chain == 0) { src = (wsel < 3 ? Wih1 : Whh1) + r * H + j; stride = H; }
-        else if (wsel < 3) { src = Wih0 + r * (A + H) + j; stride = A + H; }
+        if (chain == 0) { src = (ih ? Wih1 : Whh1) + r * H + j; stride = H; }
+        else if (ih) { src = Wih0 + r * (A + H) + j; stride = A + H; }
         else { src = Whh0 + r * H + j; stride = H; }
-      } else if (chain == 1 && row >= tg.P6) {
-        const int rr = row - tg.P6, gq = rr / 16, lr = rr % 16;
-        if (lr < U) { src = Mfold + ((size_t)(1 + gq) * H + k0) * H + c * U + lr; stride = H; }
-        else if (lr >= 8 && lr < 11) { src = Wih0 + (size_t)(gq * H + k0) * (A + H) + H + P_OUT + (lr - 8); stride = A + H; }
+      } else if (chain == 1) {
+        const int f = (row - N2) / FG, lr = (row - N2) % FG, gq = rk + f;
+        if (lr < 2 * U) { src = Mfold + ((size_t)(1 + gq) * H + k0) * H + p * 2 * U + lr; stride = H; }
+        else if (lr < 2 * U + 3) { src = Wih0 + (size_t)(gq * H + k0) * (A + H) + H + P_OUT + (lr - 2 * U); stride = A + H; }
       } else if (chain == 2) {
         if (row < U) { src = Mfold + (size_t)k0 * H + c * U + row; stride = H; }
         else if (row >= 8 && row < 11) { src = W0 + (size_t)k0 * A + P_OUT + (row - 8); stride = A; }
@@ -111,8 +124,8 @@ inline BtWs make_btws(void* base, const DecGeom& g) {
   w.bytes = off; return w;
 }
 
-#define BTDBG1(ev) do { if (iw.dbg && c == 1 && lane == 0 && (T - 1 - t) < 64) iw.dbg[(T - 1 - t) * 32 + (ev)] = clock64(); } while (0)
-#define BTDBG(ev) do { if (iw.dbg && c == 0 && lane == 0 && (T - 1 - t) < 64) iw.dbg[(T - 1 - t) * 32 + (ev)] = clock64(); } while (0)
+// trace of CTAs 0 and 1 (both ranks of pair 0): dbg[c][reverse step < 64][event < 32], clock64 of the CTA's SM
+#define BTDBG(ev) do { if (iw.dbg && c < 2 && lane == 0 && (T - 1 - t) < 64) iw.dbg[c * 2048 + (T - 1 - t) * 32 + (ev)] = clock64(); } while (0)
 
 // store U bf16 values at (row, k = j0..j0+U-1) of an image with `rows`-row tiles
 template <int U>
@@ -126,14 +139,21 @@ __device__ __forceinline__ void store_img_row(uint8_t* img, int rows, int row, i
 }
 
 // Warp roles (224 threads): warps 0..3 = the MMA warpgroup, warp 4 = epilogue (lane = sample), warp 5 = weight producer (runs
-// ahead across barriers), warp 6 = activation loader (grid-barrier waiter; streams the A images through the ring).  A chain's
-// accumulator D[128 x N] is two m64 wgmma accumulators in the warpgroup's registers; once the chain has completed they are staged
-// in shared memory (column-major, BT_ACC_LD floats per column) and the epilogue adds up the block-diagonal entries from there.
+// ahead across barriers), warp 6 = activation loader (grid-barrier waiter; streams the rank's half of the A images through the
+// ring).  A chain's accumulator D[64 x N] is one m64 wgmma accumulator in the warpgroup's registers; once the chain has completed
+// it is staged in this stage's buffer in shared memory (column-major, BT_ACC_LD floats per column), the local epilogue and the
+// peer's are signalled, and each adds up the block-diagonal entries for its own units from both ranks' buffers.
+//
+// Reusing a stage buffer across reverse steps is race-free: the buffer of stage s is rewritten at step t-1 only after that
+// step's chain s has consumed its image, which the loader streams only after a grid barrier that every CTA's epilogue arrives
+// at after its stage-s reads of step t: the G1 image of t-1 (for B2) after the B4 epilogue of t, the G0 image (B3) after the
+// B2 epilogue of t-1, the dpa image (B4) after the B3 epilogue of t-1.  The same ordering keeps a rank's remote arrival on
+// d_full[s] for step t-1 behind the epilogue's wait on it for step t, so no phase of d_full completes early.
 template <int U>
 __global__ void __launch_bounds__(224, 1)
 decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg, DecWs w, BwdWs bw, BtWs iw, BwdArgsDev d,
                       const uint8_t* __restrict__ packed) {
-  constexpr int P6 = (6 * U + 15) / 16 * 16, N2 = P6, N3 = P6 + 48, N4 = 16;
+  constexpr int N2 = 6 * U, FG = (2 * U + 3 + 7) / 8 * 8, N3A = N2 + FG, N3B = N2 + 2 * FG, N4 = 16;
   constexpr int LD = BT_ACC_LD;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -141,21 +161,24 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
   uint8_t* tail = ring + (size_t)BT_RING * tg.slot_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(tail);           // [BT_RING]  two producers (activations, weights) arrive on each
   uint64_t* empty = full + BT_RING;                             // [BT_RING]  one arrival per MMA warp
-  uint64_t* d_full = empty + BT_RING;                           // [3]
-  float* accs = reinterpret_cast<float*>(tail + 512);           // [N3][LD]  staged accumulator of the last chain
-  float* c_w2r = accs + N3 * LD;                                // [6][U]  W2[n][j] * out_std[n], n < 6, this CTA's units
+  uint64_t* d_full = empty + BT_RING;                           // [3]  B2, B3: this rank's and the peer's publish; B4: this rank's
+  float* acc2 = reinterpret_cast<float*>(tail + 512);           // [N2][LD]   staged B2 accumulator (read by both ranks)
+  float* acc3 = acc2 + N2 * LD;                                 // [N3B][LD]  staged B3 accumulator (read by both ranks)
+  float* acc4 = acc3 + N3B * LD;                                // [N4][LD]   staged B4 accumulator (rows 0..31)
+  float* c_w2r = acc4 + N4 * LD;                                // [6][U]  W2[n][j] * out_std[n], n < 6, this CTA's units
   float* c_gis = c_w2r + 6 * U;                                 // [4]     1 / in_std of the gaze channels
 
   // warp index broadcast from lane 0: provably warp-uniform, so the role branches below do not count as divergent code for wgmma
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int c = blockIdx.x, H = a.H, T = a.T;
+  const int rk = c & 1, peer = rk ^ 1;                          // rank in the cluster (clusters of 2 along x)
   const int kbH = tg.kbH;
   const uint8_t* pk = packed + (size_t)c * tg.cta_bytes;
   constexpr int W_EPI = 4, W_PROD = 5, W_LOAD = 6;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < BT_RING; ++i) { mbar_init(&full[i], 2); mbar_init(&empty[i], 4); }
-    for (int i = 0; i < 3; ++i) mbar_init(&d_full[i], 1);
+    mbar_init(&d_full[0], 2); mbar_init(&d_full[1], 2); mbar_init(&d_full[2], 1);
     fence_mbar_init();
   }
   if (threadIdx.x < 6 * U) {
@@ -163,7 +186,7 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
     c_w2r[threadIdx.x] = a.W2[(size_t)n * H + c * U + u] * a.out_std[n];
   }
   if (threadIdx.x < 3) c_gis[threadIdx.x] = 1.0f / a.in_std[P_OUT + threadIdx.x];
-  __syncthreads();
+  cluster_sync_all();                                           // both ranks' mbarriers are initialised before any remote arrive
   const size_t actH = (size_t)g.nbt * H * 32, act3 = (size_t)g.nbt * 3 * H * 32, act4 = (size_t)g.nbt * 4 * H * 32;
 
   if (warp == W_PROD) {
@@ -182,34 +205,37 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
         }
       };
       for (int t = T - 1; t >= 1; --t) {
-        stream(0, kbH, tg.N2, 2); stream(1, kbH, tg.N3, 2);
-        if (t > 1) stream(2, kbH, tg.N4, 8);
+        stream(0, kbH, tg.N2, 2); stream(1, kbH, tg.N3[rk], 2);
+        if (t > 1) stream(2, kbH, tg.N4, 4);
       }
     }
   } else if (warp == W_LOAD) {
-    // ================= activation loader
+    // ================= activation loader: per k-block, the rank's 64-row half of a 128-row tile (8 KB, contiguous: the SW128
+    // swizzle depends on row & 7 only) or a whole 32-row tile
     if (lane == 0) {
       uint32_t it = 0; unsigned epoch = 0;
       int t = T - 1; int sidx = 0;
-      auto stream = [&](const uint8_t* img, int nkb, uint32_t tile_bytes) {
+      auto stream = [&](const uint8_t* img, int nkb, uint32_t tile_bytes, uint32_t part_bytes, uint32_t part_off) {
         grid_wait(bw.bar, (++epoch) * gridDim.x);
-        if (iw.dbg && c == 0 && (T - 1 - t) < 64) iw.dbg[(T - 1 - t) * 32 + 2 * (sidx & 3)] = clock64();
+        if (iw.dbg && c < 2 && (T - 1 - t) < 64) iw.dbg[c * 2048 + (T - 1 - t) * 32 + 2 * (sidx & 3)] = clock64();
         ++sidx;
         fence_proxy_async();
-        const int kps = BT_XPART / (int)tile_bytes;               // 2 k-blocks of a 128-row image, 8 of a 32-row image
+        const int kps = BT_XPART / (int)part_bytes;               // 2 k-blocks of a 128-row image, 4 of a 32-row image
         for (int kb = 0; kb < nkb; kb += kps, ++it) {
           const uint32_t s = it % BT_RING, ph = (it / BT_RING) & 1;
-          const uint32_t bytes = (uint32_t)min(kps, nkb - kb) * tile_bytes;
+          const int nk = min(kps, nkb - kb);
           mbar_wait(&empty[s], ph ^ 1);
-          mbar_arrive_expect_tx(&full[s], bytes);
-          bulk_g2s(ring + (size_t)s * tg.slot_bytes, img + (size_t)kb * tile_bytes, bytes, &full[s]);
+          mbar_arrive_expect_tx(&full[s], (uint32_t)nk * part_bytes);
+          for (int kk = 0; kk < nk; ++kk)
+            bulk_g2s(ring + (size_t)s * tg.slot_bytes + (size_t)kk * part_bytes, img + (size_t)(kb + kk) * tile_bytes + part_off,
+                     part_bytes, &full[s]);
         }
       };
       for (t = T - 1; t >= 1; --t) {
         sidx = 0;
-        stream(iw.g1img, kbH, 16384); BTDBG(3);
-        stream(iw.g0img, kbH, 16384); BTDBG(5);
-        if (t > 1) { stream(iw.dpaimg, kbH, 4096); BTDBG(7); }
+        stream(iw.g1img, kbH, 16384, 8192, rk * 8192); BTDBG(3);
+        stream(iw.g0img, kbH, 16384, 8192, rk * 8192); BTDBG(5);
+        if (t > 1) { stream(iw.dpaimg, kbH, 4096, 4096, 0); BTDBG(7); }
       }
     }
   } else if (warp < 4) {
@@ -217,11 +243,10 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
     uint32_t it = 0;
     const uint64_t dR = make_smem_desc_sw128(ring);
     const uint32_t sstep = (uint32_t)(tg.slot_bytes >> 4);
-    float d2[2][N2 / 2], d3[2][N3 / 2], d4[2][N4 / 2];
-    // rows 64..127 of a 128-row image tile are 8 KB past its base; `two` = both row halves (128-row images) or rows 0..63 only
-    auto chain_mma = [&](auto& dd, auto two, int nkb, int kps, uint32_t atile) {
-      constexpr int N = 2 * (int)(sizeof(dd[0]) / sizeof(float));
-      constexpr bool TWO = decltype(two)::value;
+    float d2[N2 / 2], d3a[N3A / 2], d3b[N3B / 2], d4[N4 / 2];
+    // a 32-row B4 tile feeds the m64 MMA rows 32..63 from whatever follows it in the slot: they are never staged
+    auto chain_mma = [&](auto& dd, int nkb, int kps, uint32_t atile, float* out, int nrows) {
+      constexpr int N = 2 * (int)(sizeof(dd) / sizeof(float));
       const uint32_t astep = atile >> 4, wstep = (uint32_t)(N * 128) >> 4;
       uint32_t prev = 0;
       for (int kb = 0; kb < nkb; kb += kps, ++it) {
@@ -232,11 +257,7 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
         wgmma_fence();
         for (int kk = 0; kk < nk; ++kk, da += astep, db += wstep) {
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint32_t acc = (kb + kk + ks) > 0 ? 1u : 0u;
-            Wgmma<N>::mma(dd[0], da + 2 * ks, db + 2 * ks, acc);
-            if constexpr (TWO) Wgmma<N>::mma(dd[1], da + 512 + 2 * ks, db + 2 * ks, acc);
-          }
+          for (int ks = 0; ks < 4; ++ks) Wgmma<N>::mma(dd, da + 2 * ks, db + 2 * ks, (kb + kk + ks) > 0 ? 1u : 0u);
         }
         wgmma_commit();
         if (kb > 0) {
@@ -246,28 +267,35 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
         prev = s;
       }
       wgmma_wait<0>();
-      wgmma_fence_operands(dd[0]);
-      if (TWO) wgmma_fence_operands(dd[1]);
+      wgmma_fence_operands(dd);
       if (lane == 0) mbar_arrive(&empty[prev]);
-      stage_acc<N>(dd[0], accs, LD, 0, TWO ? 64 : 32);
-      if constexpr (TWO) stage_acc<N>(dd[1], accs, LD, 64, 64);
+      stage_acc<N>(dd, out, LD, 0, nrows);
     };
+    // B2 / B3 buffers are read by both ranks: the peer is signalled with a cluster-scope release after the staging barrier
     auto publish = [&](int i) {
       named_bar(1, 128);
-      if (threadIdx.x == 0) mbar_arrive(&d_full[i]);
+      if (threadIdx.x == 0) {
+        mbar_arrive(&d_full[i]);
+        if (i < 2) mbar_arrive_cluster(&d_full[i], (uint32_t)peer);
+      }
     };
     for (int t = T - 1; t >= 1; --t) {
-      chain_mma(d2, std::true_type(), kbH, 2, 16384); publish(0); BTDBG(9);
-      chain_mma(d3, std::true_type(), kbH, 2, 16384); publish(1); BTDBG(10);
-      if (t > 1) { chain_mma(d4, std::false_type(), kbH, 8, 4096); publish(2); BTDBG(11); }
+      chain_mma(d2, kbH, 2, 8192, acc2, 64); publish(0); BTDBG(9);
+      if (rk == 0) chain_mma(d3a, kbH, 2, 8192, acc3, 64);
+      else chain_mma(d3b, kbH, 2, 8192, acc3, 64);
+      publish(1); BTDBG(10);
+      if (t > 1) { chain_mma(d4, kbH, 4, 4096, acc4, 32); publish(2); BTDBG(11); }
     }
   } else if (warp == W_EPI) {
-    // ================= epilogue (lane = sample b).  Row 32*blk + b of a staged 128-row accumulator is block blk of sample b:
-    // B2 / B3 blocks pr, pz, pn, pnr pair with the weight column groups (ih_r, hh_r), (ih_z, hh_z), (ih_n, -), (-, hh_n).
+    // ================= epilogue (lane = sample b).  Row 32*blk + b of a staged B2 / B3 accumulator is local block blk of sample
+    // b: rank 0 holds pr, pnr, rank 1 pz, pn.  Column grp * 2U + wo + u is unit u of this CTA in gate group grp (wo = rk * U).
     const int b = lane;
     const bool live = b < a.B;
-    const int j0 = c * U;
-    auto A = [&](int col, int blk) { return accs[(size_t)col * LD + 32 * blk + b]; };
+    const int j0 = c * U, wo = rk * U;
+    // shared::cluster addresses of rank 0's and rank 1's B2 buffer (acc3 = acc2 + N2 * LD in both CTAs)
+    const uint32_t a2r0 = cluster_map(acc2, 0u), a2r1 = cluster_map(acc2, 1u);
+    auto X = [&](uint32_t s, int col, int blk) { return ld_cluster_f32(s + (uint32_t)(col * LD + 32 * blk + b) * 4u); };
+    auto A = [&](const float* s, int col, int blk) { return s[(size_t)col * LD + 32 * blk + b]; };
     // ---- R(t): adjoint of the root integration of frame t and of the gaze direction of step t+1 (modules.py:696, :739-740),
     // run by EVERY CTA for the 32 samples (lane = sample).  Returns dch[0:6] = d loss / d (de-normalised y(t)[0:6])
     // through the root chain and advances the running d root_pos / d root_rot.
@@ -341,7 +369,7 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
       dpq[5] = dq_a.y + dq_b.y + dq_c.y + e1q[2]; dpq[6] = dq_a.z + dq_b.z + dq_c.z + e1q[3];
     };
     // ---- GRU layer-1 gate adjoint of frame t from dh1(t): writes the G1 image + histories, keeps dh1*z
-    float dhz1[U], dhz0[U], dsum[16];
+    float dhz1[U], dhz0[U], dsf[U], dsg[3];
     float g1r[U], g1z[U], g1n[U], g1hn[U], g1hp[U], g1acc[U], prev[U];
     auto G1_prefetch = [&](int t) {
       const float* G = w.G1 + t * act4;
@@ -371,8 +399,8 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
         gru_gate_bwd(dh, g1r[u], g1z[u], g1n[u], g1hn[u], g1hp[u], dgi, dgh, dhz1[u]);
         pr[u] = dgi[0]; pz[u] = dgi[1]; pn[u] = dgi[2]; pnr[u] = dgh[2];
       }
-      store_img_row<U>(iw.g1img, 128, 0 * 32 + b, j0, pr); store_img_row<U>(iw.g1img, 128, 1 * 32 + b, j0, pz);
-      store_img_row<U>(iw.g1img, 128, 2 * 32 + b, j0, pn); store_img_row<U>(iw.g1img, 128, 3 * 32 + b, j0, pnr);
+      store_img_row<U>(iw.g1img, 128, 0 * 32 + b, j0, pr); store_img_row<U>(iw.g1img, 128, 1 * 32 + b, j0, pnr);
+      store_img_row<U>(iw.g1img, 128, 2 * 32 + b, j0, pz); store_img_row<U>(iw.g1img, 128, 3 * 32 + b, j0, pn);
       grid_arrive(bw.bar);
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -414,21 +442,21 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
           acc[u] = t == T - 1 ? 0.f : bw.DH0[(size_t)j * 32 + b];
         }
       }
-      mbar_wait(&d_full[0], ph);
+      mbar_wait_cluster(&d_full[0], ph);
       BTDBG(14);
       {
         float pr[U], pz[U], pn[U], pnr[U], dh1n[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-          const float oa = (A(0 * U + u, 0) + A(1 * U + u, 1)) + A(2 * U + u, 2);     // W_ih1^T dgi1
-          const float ob = (A(3 * U + u, 0) + A(4 * U + u, 1)) + A(5 * U + u, 3);     // W_hh1^T dgh1
+          const float oa = (X(a2r0, 0 * 2 * U + wo + u, 0) + X(a2r1, 0 * 2 * U + wo + u, 0)) + X(a2r1, 2 * 2 * U + wo + u, 1);  // W_ih1^T dgi1
+          const float ob = (X(a2r0, 1 * 2 * U + wo + u, 0) + X(a2r1, 1 * 2 * U + wo + u, 0)) + X(a2r0, 2 * 2 * U + wo + u, 1);  // W_hh1^T dgh1
           float dgi[3], dgh[3];
           gru_gate_bwd(oa + acc[u], gr[u], gz[u], gn[u], ghn[u], hp[u], dgi, dgh, dhz0[u]);
           pr[u] = dgi[0]; pz[u] = dgi[1]; pn[u] = dgi[2]; pnr[u] = dgh[2];
           dh1n[u] = ob + dhz1[u];                                         // dh1(t-1) = dh1*z1 + W_hh1^T dgh1 (+ fold terms at B4)
         }
-        store_img_row<U>(iw.g0img, 128, 0 * 32 + b, j0, pr); store_img_row<U>(iw.g0img, 128, 1 * 32 + b, j0, pz);
-        store_img_row<U>(iw.g0img, 128, 2 * 32 + b, j0, pn); store_img_row<U>(iw.g0img, 128, 3 * 32 + b, j0, pnr);
+        store_img_row<U>(iw.g0img, 128, 0 * 32 + b, j0, pr); store_img_row<U>(iw.g0img, 128, 1 * 32 + b, j0, pnr);
+        store_img_row<U>(iw.g0img, 128, 2 * 32 + b, j0, pz); store_img_row<U>(iw.g0img, 128, 3 * 32 + b, j0, pn);
         BTDBG(16);
         grid_arrive(bw.bar);
 #pragma unroll
@@ -446,20 +474,23 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
       float av[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) av[u] = w.A[t * actH + (size_t)(j0 + u) * 32 + b];
-      mbar_wait(&d_full[1], ph);
+      mbar_wait_cluster(&d_full[1], ph);
       BTDBG(17);
       {
         float dpa[U], dh0n[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-          const float da = (A(0 * U + u, 0) + A(1 * U + u, 1)) + A(2 * U + u, 2);
-          const float ob = (A(3 * U + u, 0) + A(4 * U + u, 1)) + A(5 * U + u, 3);
+          const float da = (X(a2r0, N2 + 0 * 2 * U + wo + u, 0) + X(a2r1, N2 + 0 * 2 * U + wo + u, 0)) + X(a2r1, N2 + 2 * 2 * U + wo + u, 1);
+          const float ob = (X(a2r0, N2 + 1 * 2 * U + wo + u, 0) + X(a2r1, N2 + 1 * 2 * U + wo + u, 0)) + X(a2r0, N2 + 2 * 2 * U + wo + u, 1);
           dpa[u] = da * (av[u] > 0.f ? 1.f : av[u] + 1.f);                 // ELU'(pre) = a + 1 for pre <= 0
           dh0n[u] = ob + dhz0[u];
         }
+        // fold groups r (rank 0), z, n (rank 1): Mfold^T dgi0 for this CTA's units, and the gaze adjoint (columns 2U..2U+2)
 #pragma unroll
-        for (int r = 0; r < 16; ++r)          // gate blocks of Mfold^T dgi0 (cols 0..U-1) and of the gaze adjoint (cols 8..10)
-          dsum[r] = (A(P6 + r, 0) + A(P6 + 16 + r, 1)) + A(P6 + 32 + r, 2);
+        for (int u = 0; u < U; ++u) dsf[u] = (X(a2r0, N2 + N2 + wo + u, 0) + X(a2r1, N2 + N2 + wo + u, 0)) + X(a2r1, N2 + N2 + FG + wo + u, 1);
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+          dsg[i] = (X(a2r0, N2 + N2 + 2 * U + i, 0) + X(a2r1, N2 + N2 + 2 * U + i, 0)) + X(a2r1, N2 + N2 + FG + 2 * U + i, 1);
         store_img_row<U>(iw.dpaimg, 32, b, j0, dpa);
         BTDBG(18);
         if (t > 1) grid_arrive(bw.bar);
@@ -471,19 +502,17 @@ decoder_bwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, BtGeom tg
       R_prefetch(t - 1, true); R_precompute(); G1_prefetch(t - 1);
       mbar_wait(&d_full[2], ph);
       BTDBG(19);
-      float tot[16];
-#pragma unroll
-      for (int r = 0; r < 16; ++r) tot[r] = A(r, 0) + dsum[r];
       float fold[U], dgz[3], dch[6];
 #pragma unroll
-      for (int u = 0; u < U; ++u) fold[u] = tot[u];
+      for (int u = 0; u < U; ++u) fold[u] = A(acc4, u, 0) + dsf[u];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) dgz[i] = tot[8 + i] * c_gis[i];          // modules.py:713 (x = (gaze_dir - mean) / std)
+      for (int i = 0; i < 3; ++i) dgz[i] = (A(acc4, 8 + i, 0) + dsg[i]) * c_gis[i];   // modules.py:713 (x = (gaze_dir - mean) / std)
       R_adjoint(dgz, true, dch);
       BTDBG(20);
       G1_adjoint(t - 1, fold, dch);
     }
   }
+  cluster_sync_all();           // a CTA's shared memory must outlive the peer's last reads of its staged accumulators
 }
 
 // ------------------------------------------------------------------ host
@@ -527,19 +556,30 @@ extern "C" int zeggs_decoder_pack_weights_bwd_tc(const zeggs_decoder_fwd_args* a
 template <int U>
 static int launch_bt(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdGeom& bg, const BtGeom& tg, const DecWs& w,
                      const BwdWs& bw, const BtWs& iw, const BwdArgsDev& d, const uint8_t* packed, cudaStream_t stream) {
-  const size_t smem = 1024 + (size_t)BT_RING * tg.slot_bytes + 512 + (size_t)(tg.N3 * BT_ACC_LD + 6 * U + 16) * sizeof(float);
-  static size_t checked_smem = 0;     // attribute + co-residency check once per shared-memory size (one device per process)
+  const size_t smem = 1024 + (size_t)BT_RING * tg.slot_bytes + 512 +
+                      (size_t)((tg.N2 + tg.N3[1] + tg.N4) * BT_ACC_LD + 6 * U + 16) * sizeof(float);
+  // clusters of 2 CTAs (the pairs sharing an image), launched cooperatively: the kernel spins on a grid barrier, so every
+  // CTA must be resident at once
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeCooperative;
+  attr[1].val.cooperative = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(g.G); cfg.blockDim = dim3(224); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cfg.attrs = attr; cfg.numAttrs = 2;
+  static size_t checked_smem = 0;     // attribute + co-residency query once per shared-memory size (one device per process)
+  static int max_clusters = 0;
   if (checked_smem != smem) {
     ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_tc_kernel<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, nsm = 0, occ = 0;
-    ZCHECK_CUDA(cudaGetDevice(&dev));
-    ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-    ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_bwd_tc_kernel<U>, 224, smem));
-    ZCHECK_ARG(occ * nsm >= g.G, "decoder bwd tc: cooperative grid of %d CTAs does not fit", g.G);
+    cudaLaunchConfig_t occ = cfg;
+    occ.numAttrs = 1;                 // the cluster shape only
+    ZCHECK_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, decoder_bwd_tc_kernel<U>, &occ));
     checked_smem = smem;
   }
-  void* args[] = {(void*)&a, (void*)&g, (void*)&bg, (void*)&tg, (void*)&w, (void*)&bw, (void*)&iw, (void*)&d, (void*)&packed};
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_bwd_tc_kernel<U>, dim3(g.G), dim3(224), args, smem, stream));
+  ZCHECK_ARG(2 * max_clusters >= g.G, "decoder bwd tc: cooperative grid of %d CTAs in clusters of 2 does not fit (%d clusters resident)",
+             g.G, max_clusters);
+  ZCHECK_CUDA(cudaLaunchKernelEx(&cfg, decoder_bwd_tc_kernel<U>, a, g, bg, tg, w, bw, iw, d, packed));
   count_launch();
   return ZEGGS_OK;
 }

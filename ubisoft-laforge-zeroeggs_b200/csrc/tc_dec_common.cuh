@@ -17,17 +17,40 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// ---- thread-block clusters: rank / size, cluster barrier, multicast bulk copy (one L2 read feeds every CTA of the cluster)
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t cluster_nctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctarank;\n" : "=r"(r)); return r; }
+// ---- thread-block clusters: cluster barrier, distributed shared memory (DSMEM), mbarrier signals across the cluster
+// every thread of every CTA of the cluster; not .aligned, so the threads of a warp may arrive from different branches
 __device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+  asm volatile("barrier.cluster.arrive.release;\n" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire;\n" ::: "memory");
 }
-// the copy lands at the same shared-memory offset in every CTA of `mask` and completes `bytes` on each one's mbarrier
-__device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint16_t mask) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;\n"
-               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "h"(mask) : "memory");
+// shared::cluster address of the same shared-memory object in CTA `rank` of the cluster, and a load through such an address
+// (volatile: it stays after the mbarrier wait that publishes the data)
+__device__ __forceinline__ uint32_t cluster_map(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ float ld_cluster_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];\n" : "=f"(v) : "r"(addr));
+  return v;
+}
+// arrive on the mbarrier at `bar`'s offset in CTA `rank`; release at cluster scope: this thread's earlier shared-memory writes,
+// and those ordered before them by a CTA barrier, are visible to a thread that then acquires the phase with mbar_wait_cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_map(bar, rank)) : "memory");
+}
+// mbar_wait with acquire at cluster scope (the phase includes arrivals from another CTA of the cluster)
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  const uint32_t addr = smem_u32(bar);
+  uint32_t done = 0;
+#pragma unroll 1
+  for (uint32_t it = 0; it < 20000000u; ++it) {
+    asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}\n"
+                 : "=r"(done) : "r"(addr), "r"(parity) : "memory");
+    if (done) return;
+  }
+  __trap();
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;\n" ::: "memory"); }
 
