@@ -354,32 +354,36 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
     return grads, dSpeech, dStyle, finish
 
 
-def loss_fwd_bwd(Y, rp, rq, WY, Wrp, Wrq, gaze, parents_i32, dt, mu, logvar, kl_weight, terms_out=None, kl_weight_dev=None):
-    """train.py:277-421 forward and gradient in one call (zeggs_loss_fwd_bwd) -> (loss = terms[0], (dY, dRp, dRq, dmu, dlogvar))."""
+def loss_fwd_bwd(Y, rp, rq, WY, Wrp, Wrq, gaze, parents_i32, dt, mu, logvar, kl_weight, terms_out=None, kl_weight_dev=None, grad=True):
+    """train.py:277-421 forward and gradient in one call (zeggs_loss_fwd_bwd) -> (loss = terms[0], (dY, dRp, dRq, dmu, dlogvar)).
+    grad=False: the 19 terms only (dY == NULL: no backward kernels) -> (loss, None)."""
     l = _lib.lib()
     dev = Y.device
     B, T = Y.shape[0], Y.shape[1]
     f = _f32c
     Y, rp, rq, WY, Wrp, Wrq, gaze = f(Y), f(rp), f(rq), f(WY), f(Wrp), f(Wrq), f(gaze)
     losses = terms_out if terms_out is not None else torch.empty(19, dtype=torch.float32, device=dev)
-    dY, dRp, dRq = torch.empty_like(Y), torch.empty_like(rp), torch.empty_like(rq)
     a = _lib.LossArgs(B=B, T=T, Z=(mu.shape[1] if mu is not None else 0), dt=dt, kl_weight=kl_weight)
     if kl_weight_dev is not None:          # device scalar (graph-replayable): overrides the by-value weight
         a.kl_weight_dev = kl_weight_dev.data_ptr()
     a.Y, a.root_pos, a.root_rot = Y.data_ptr(), rp.data_ptr(), rq.data_ptr()
     a.WY, a.W_root_pos, a.W_root_rot = WY.data_ptr(), Wrp.data_ptr(), Wrq.data_ptr()
     a.gaze_pos, a.parents, a.losses = gaze.data_ptr(), parents_i32.data_ptr(), losses.data_ptr()
-    a.dY, a.dRootPos, a.dRootRot = dY.data_ptr(), dRp.data_ptr(), dRq.data_ptr()
+    if grad:
+        dY, dRp, dRq = torch.empty_like(Y), torch.empty_like(rp), torch.empty_like(rq)
+        a.dY, a.dRootPos, a.dRootRot = dY.data_ptr(), dRp.data_ptr(), dRq.data_ptr()
     dmu = dlv = None
     if mu is not None:
         mu, logvar = f(mu), f(logvar)
-        dmu, dlv = torch.empty_like(mu), torch.empty_like(logvar)
-        a.mu, a.logvar, a.dmu, a.dlogvar = mu.data_ptr(), logvar.data_ptr(), dmu.data_ptr(), dlv.data_ptr()
+        a.mu, a.logvar = mu.data_ptr(), logvar.data_ptr()
+        if grad:
+            dmu, dlv = torch.empty_like(mu), torch.empty_like(logvar)
+            a.dmu, a.dlogvar = dmu.data_ptr(), dlv.data_ptr()
     wsb = l.zeggs_loss_workspace_bytes(B, T)
     ws = WS.get("loss", wsb, dev)
     a.workspace, a.workspace_bytes = ws.data_ptr(), wsb
     _lib.check(l.zeggs_loss_fwd_bwd(a, _lib.stream_ptr()), "zeggs_loss_fwd_bwd")
-    return losses[0], (dY, dRp, dRq, dmu, dlv)
+    return losses[0], ((dY, dRp, dRq, dmu, dlv) if grad else None)
 
 
 def decoder_window(dec, root_pos0, root_rot0, pose0, gaze_pos, speech, style,

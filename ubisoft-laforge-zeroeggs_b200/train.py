@@ -17,6 +17,9 @@ from . import _lib, dp, modules, ops
 from .optimizers import RAdam
 
 POSE_KEYS = ["root_pos", "root_rot", "root_vel", "root_vrt", "lpos", "ltxy", "lvel", "lvrt"]
+# the 19 entries of the loss vector (TrainStep.terms, TrainStep.evaluate): the total, the 17 L1 terms of train.py:340-395, the weighted KL
+TERM_NAMES = ["total", "root_pos", "root_rot", "root_vel", "root_vrt", "lpos", "lrot", "lvel", "lvrt", "cpos", "crot", "cvel", "cvrt",
+              "ldvl", "ldvt", "cdvl", "cdvt", "gaze", "kl_div"]
 
 
 def kl_weight(iteration, center=7500, rate=0.005, threshold=0.2):
@@ -57,7 +60,7 @@ class TrainStep:
     all-reduce of the flat gradient -> graph B (RAdam)."""
 
     def __init__(self, speech_encoder, decoder, style_encoder, stats, parents, dt, lr=1e-4, eps=1e-5,
-                 world_size=1, process_group=None, use_graph=False):
+                 world_size=1, process_group=None, use_graph=False, eval_seed=0):
         parents = check_parents(parents)          # before anything reaches the device
         self.se, self.dec, self.st = speech_encoder, decoder, style_encoder
         self.dev = next(decoder.parameters()).device
@@ -78,6 +81,7 @@ class TrainStep:
         self.klw = torch.zeros(1, dtype=torch.float32, device=self.dev)      # annealed KL weight, device scalar
         self.use_graph = bool(use_graph)
         self.seed = ops.DeviceSeed(self.dev) if self.use_graph else None
+        self.eval_seed = int(eval_seed)     # VAE noise of evaluate(): its own generator, re-seeded per call (see evaluate)
         self._graphs, self._seen, self._pool = {}, {}, None
         self.graph_min_seen = 1            # eager steps on a new batch geometry before it is captured
         self.graph_launches = 0            # library launches captured per replay (gpu_launches accounting)
@@ -177,6 +181,39 @@ class TrainStep:
         del keep
         return loss
 
+    @torch.no_grad()
+    def evaluate(self, batch, eps=None, index=0):
+        """Forward only, in eval mode (no dropout): encoders -> decoder window -> the fused loss without its backward.  Returns the
+        19 loss terms (TERM_NAMES) as a new device tensor, weighted with the same kl_weight(iteration) as training.
+        The VAE noise is `eps` if given, else drawn from a generator seeded with (eval_seed, index) -- so the same weights and batch
+        give bitwise-identical terms on every call.  Leaves the flat gradient, the optimizer state, `iteration`, `terms`, the
+        dropout DeviceSeed, torch's / numpy's / Python's global generators and the captured training graphs alone."""
+        se, dec, st = self.se, self.dec, self.st
+        with eval_mode(se, dec, st):
+            xa = ops.normalize_rows(batch["audio"], self.audio_mean, self.audio_std)
+            speech, _ = ops.speech_encoder_fwd(se, xa, None)
+            mu = logvar = None
+            if st is not None:
+                xs = ops.normalize_rows(batch["style"], self.in_mean, self.in_std)
+                if eps is None and st.use_vae:
+                    g = torch.Generator(device=self.dev)
+                    g.manual_seed(self.eval_seed * 1000003 + int(index))
+                    eps = torch.randn((xs.shape[0], dec.style_encoding_size), generator=g, device=self.dev)
+                eps_, _ = ops.style_encoder_prepare(st, xs, eps, None)
+                (z, mu, logvar), _ = ops.style_encoder_fwd(st, xs, eps_, None, 1.0)
+            else:
+                z = batch["style"]
+            T = speech.shape[1]
+            W = [batch[k] for k in POSE_KEYS]
+            WY = pack_pose(*W[2:])
+            Y, rp, rq, _ = ops.decoder_window_forward(dec, W[0][:, 0], W[1][:, 0], WY[:, 0], batch["gaze_pos"], speech,
+                                                      z.unsqueeze(1).expand(-1, T, -1),
+                                                      (self.in_mean, self.in_std, self.out_mean, self.out_std), self.dt, save=False)
+            terms = torch.empty(19, dtype=torch.float32, device=self.dev)
+            ops.loss_fwd_bwd(Y, rp, rq, WY, W[0], W[1], batch["gaze_pos"], self.parents, self.dt, mu, logvar,
+                             kl_weight(self.iteration) if mu is not None else 0.0, terms, grad=False)
+        return terms
+
     def _allreduce(self):
         if self.ar_events is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -264,6 +301,83 @@ class TrainStep:
         return self._graphs[key]
 
 
+class eval_mode:
+    """Networks in eval mode for the block, restored afterwards together with their cached weight packs (`_zeggs_*`).  The packs a
+    captured training graph writes were allocated in the graph's private memory pool; an eager call that re-packs would drop the
+    module's last reference to them, and a later capture could then hand that memory to something else while the first graph still
+    writes it.  Restoring keeps them referenced (their version keys are stale, so the next eager call packs afresh)."""
+
+    def __init__(self, *nets):
+        self.nets = [m for m in nets if m is not None]
+
+    def __enter__(self):
+        self.state = [(m, m.training, {k: v for k, v in m.__dict__.items() if k.startswith("_zeggs")}) for m in self.nets]
+        for m in self.nets:
+            m.eval()
+        return self
+
+    def __exit__(self, *exc):
+        for m, training, caches in self.state:
+            m.train(training)
+            m.__dict__.update(caches)
+        return False
+
+
+def validate(stepper, ds, batchsize):
+    """Held-out loss: every validation window of `ds` (data.validation_windows) through stepper.evaluate in batches of `batchsize`
+    (the last one may be smaller).  -> (window-weighted mean of each of the 19 terms as float64 numpy [19], window count), or
+    (None, 0) without a validation split.  Every term is a mean over its batch, so weighting by window count gives the exact mean
+    over all windows."""
+    n = len(ds.valid_starts)
+    if n == 0:
+        return None, 0
+    acc = torch.zeros(19, dtype=torch.float64, device=stepper.dev)
+    for k, i in enumerate(range(0, n, batchsize)):
+        idx = np.arange(i, min(i + batchsize, n))
+        terms = stepper.evaluate(ds.valid_batch(idx, stepper.dev), index=k)
+        acc += terms.double() * len(idx)
+    return (acc / n).cpu().numpy(), n
+
+
+@torch.no_grad()
+def write_samples(samples_dir, iteration, ds, se, de, st, stats, details, style_encoding_type, rs, device, splits=("train", "valid")):
+    """train.py:511-729: for each split three clips of at most 30 s (dataset.py:206-233, ranges picked by `rs`), the networks in eval
+    mode on the clip's audio from its first pose along its gaze track, and the ground truth and the prediction written as BVH files
+    iteration_{it}_{split}_{ground|predict}_{i}_{label}.bvh.  The style is the clip's own example (get_example over the clip, the
+    current example length; VAE noise from `rs`) or its one-hot label.  File-system errors are printed, not raised (:622-623)."""
+    from . import bvhio
+    f = lambda k: torch.as_tensor(stats[k], dtype=torch.float32, device=device)
+    in_mean, in_std, out_mean, out_std = f("anim_input_mean"), f("anim_input_std"), f("anim_output_mean"), f("anim_output_std")
+    parents, names, dt = details["parents"], details["bone_names"], float(details["dt"])
+    with eval_mode(se, de, st):
+        for split in splits:
+            for i in range(3):
+                clip, label, rng, _ = ds.get_sample(split, 30, rs=rs)
+                c = {k: v.to(device) for k, v in clip.items()}
+                speech = se((c["audio"] - f("audio_input_mean")) / f("audio_input_std"))
+                if style_encoding_type == "example":
+                    ex = (ds.get_example(rng, rng, ds.example_window_length).to(device) - in_mean) / in_std
+                    eps = torch.from_numpy(rs.randn(1, de.style_encoding_size).astype(np.float32)).to(device) if st.use_vae else None
+                    z, _, _ = st(ex[None], 1.0, eps=eps)
+                else:
+                    z = torch.zeros((1, len(details["label_names"])), dtype=torch.float32, device=device)
+                    z[0, label] = 1.0
+                T = speech.shape[1]
+                V = de(*[c[k][:, 0] for k in POSE_KEYS], c["gaze_pos"], speech, z.unsqueeze(1).repeat(1, T, 1), None,
+                       in_mean, in_std, out_mean, out_std, dt)
+                V = dict(zip(POSE_KEYS, V))
+                pos, eul = ops.pose_to_bvh_channels(*[torch.cat([c[k], V[k]], 0) for k in ("root_pos", "root_rot", "lpos", "ltxy")],
+                                                    rebase=False)
+                pos, eul = pos.cpu().numpy(), eul.cpu().numpy()
+                lab = details["label_names"][label]
+                try:
+                    for j, kind in enumerate(("ground", "predict")):
+                        bvhio.save_bvh(str(Path(samples_dir) / f"iteration_{iteration}_{split}_{kind}_{i}_{lab}.bvh"), pos[j], eul[j],
+                                       parents, names, "zyx", dt)
+                except (PermissionError, OSError) as e:
+                    print(e)
+
+
 def pin_to_gpu_numa(local_rank):
     """Bind this process (the launch thread of one rank) to the CPUs of the NUMA node its GPU hangs off; returns the node or None.
     Un-pinned ranks of GPUs on the second socket otherwise enqueue from the remote socket."""
@@ -336,7 +450,8 @@ def train(models_dir, logs_dir, path_processed_data, path_data_definition, train
             if net is not None:
                 net.load_state_dict(torch.load(models_dir / f"{name}.pt", weights_only=False).state_dict())
     stepper = TrainStep(se, de, st, ds.stats, details["parents"], details["dt"], lr=train_options["learning_rate"],
-                        eps=train_options["eps"], world_size=world, use_graph=bool(train_options.get("cuda_graph", True)))
+                        eps=train_options["eps"], world_size=world, use_graph=bool(train_options.get("cuda_graph", True)),
+                        eval_seed=train_options["seed"])
     if train_options["resume"] and (models_dir / "checkpoints.pt").exists():
         ck = torch.load(models_dir / "checkpoints.pt", weights_only=False)
         stepper.iteration = ck["iteration"]
@@ -346,6 +461,10 @@ def train(models_dir, logs_dir, path_processed_data, path_data_definition, train
     batchsize = train_options["batchsize"]
     ex_len = network_options["style_encoder"]["example_length"]
     start = datetime.datetime.now()
+    samples_dir = logs_dir / "samples"
+    sample_rs = np.random.RandomState(train_options["seed"])        # range picks and VAE noise of the sample animations
+    if rank == 0:
+        samples_dir.mkdir(parents=True, exist_ok=True)
     prefetch = None if on_device else DevicePrefetcher(device)
     token = None if on_device else prefetch.upload(ds.sample_host_batch(batchsize))
     while stepper.iteration < total:
@@ -364,9 +483,31 @@ def train(models_dir, logs_dir, path_processed_data, path_data_definition, train
         if rank == 0 and (it % 100 == 0 or it == 1):
             print(f"iteration {it}/{total} loss {loss.item():.5f} elapsed {datetime.datetime.now() - start}", flush=True)
         if rank == 0 and it % train_options["generate_samples_step"] == 0:
-            save_checkpoint(models_dir, se, de, st, stepper, float(loss.item()))
+            train_loss = float(loss.item())
+            save_checkpoint(models_dir, se, de, st, stepper, train_loss)
+            save_checkpoint(models_dir / str(it), se, de, st, stepper, train_loss)             # train.py:493-509
+            monitor(stepper, ds, batchsize, it, train_loss, logs_dir, samples_dir, se, de, st, details, style_encoding_type,
+                    sample_rs, device)
     if rank == 0:
         save_checkpoint(models_dir, se, de, st, stepper, float(loss.item()))
+
+
+def monitor(stepper, ds, batchsize, it, train_loss, logs_dir, samples_dir, se, de, st, details, style_encoding_type, rs, device):
+    """What train() does at every generate_samples_step besides saving: the sample animations (train.py:511-729) and the held-out
+    loss (validate), printed and appended as one JSON line to logs_dir/valid_loss.jsonl.  Touches nothing the training reads."""
+    has_valid = len(ds.ranges_valid) > 0
+    write_samples(samples_dir, it, ds, se, de, st, ds.stats, details, style_encoding_type, rs, device,
+                  splits=("train", "valid") if has_valid else ("train",))
+    terms, n = validate(stepper, ds, batchsize)
+    if n == 0:
+        return
+    print(f"iteration {it} validation loss {terms[0]:.5f} over {n} windows (training loss {train_loss:.5f})", flush=True)
+    rec = {"iteration": it, "train_loss": train_loss, "valid": {k: float(v) for k, v in zip(TERM_NAMES, terms)}, "windows": n}
+    try:
+        with open(Path(logs_dir) / "valid_loss.jsonl", "a") as fh:
+            fh.write(json.dumps(rec) + "\n")
+    except (PermissionError, OSError) as e:
+        print(e)
 
 
 def save_checkpoint(models_dir, se, de, st, stepper, loss):
