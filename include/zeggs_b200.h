@@ -420,6 +420,71 @@ int zeggs_gemm_f32_ctx(const zeggs_ctx* ctx, int mode, int M, int N, int K, cons
                        const float* bias, float* C, int ldc, int act, int accumulate, void* stream);
 int zeggs_split_bf16(const float* x, int rows, int cols, int ld_in, void* hi, void* lo, int ld_out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Training-set construction (ZEGGS/data_pipeline.py:90-228, 412-432, 562-648; host side: zeggs_b200.data_pipeline).
+ *
+ * Per-frame animation features of one take (preprocess_animation, :90-228), float64 arithmetic, float32 outputs:
+ * Euler -> quaternion, unroll (an exact per-joint sign scan), the chains of FK that reach Spine2 / Hips / Head, the ground-projected
+ * root and its facing, the gaze target (exact median over frames), root-relative joint 0, finite-difference and helical velocities
+ * with frame 0 extrapolated from frames 1..3, and ltxy.  T >= 4.
+ *   rotations [T,J,3] f64 degrees in the file's channel order, order[i] = axis of channel i (0 x, 1 y, 2 z); positions [T,J,3] f64
+ *   parents [J] int32 on the device: parents[0] == -1 and 0 <= parents[j] < j (not checked here: the host validates it)
+ *   outputs root_pos [T,3], root_rot [T,4], root_vel [T,3], root_vrt [T,3], lpos [T,J,3], ltxy [T,J,2,3], lvel [T,J,3], lvrt [T,J,3],
+ *   gaze_pos [T,3], gaze_dir [T,3]
+ *   quat_out [T,J,4] f64 or NULL: the unrolled local quaternions (before joint 0 is made root-relative).  With positions == NULL only
+ *   these are computed (the input of the time-stretch, :423).
+ */
+typedef struct {
+  int T, J;
+  int order[3];
+  int spine2, hips, head;
+  double dt;
+  const double* rotations;
+  const double* positions;
+  const int* parents;
+  float *root_pos, *root_rot, *root_vel, *root_vrt, *lpos, *ltxy, *lvel, *lvrt, *gaze_pos, *gaze_dir;
+  double* quat_out;
+  void* workspace;
+  size_t workspace_bytes;
+} zeggs_anim_features_args;
+size_t zeggs_anim_features_workspace_bytes(int T, int J);
+int zeggs_anim_features(const zeggs_anim_features_args* a, void* stream);
+/* quat.normalize -> quat.to_euler(order) -> np.degrees (:426-427): q [n,4] f64 (w first) -> euler_deg [n,3] f64.
+ * order 0 = "zyx", 1 = "xzy" (the reference converts to no other order: ZEGGS_ERR_UNSUPPORTED). */
+int zeggs_quat_to_euler_deg(const double* q, double* euler_deg, long long n, int order, void* stream);
+
+/* Time-stretch (:415-432): griddata(arange(n), x, linspace(0, n-1, m), method="cubic") in 1-D, i.e. scipy's not-a-knot cubic
+ * spline through n uniform samples, evaluated at m points placed as np.linspace places them (the last exactly n-1).  Channels are
+ * independent.  x [n, C] f32 (in_f64 = 0) or f64 (in_f64 = 1), y [m, C] f64.  n >= 4. */
+typedef struct {
+  long long n, m;
+  int C, in_f64;
+  const void* x;
+  double* y;
+  void* workspace;
+  size_t workspace_bytes;
+} zeggs_spline_args;
+size_t zeggs_spline_resample_workspace_bytes(long long n, int C);
+int zeggs_spline_resample(const zeggs_spline_args* a, void* stream);
+
+/* Dataset statistics (:562-648): over the rows listed in `rows` (int32, device), per channel the mean and the population std, and per
+ * group the population std of all its elements pooled.  Group g is src[g] [n_rows, width[g]] f32; channels are numbered across the
+ * groups in order (mean / std [sum of widths] f64, group_std [n_groups] f64).  float64 accumulation, two passes, fixed order: a
+ * channel that is constant over the rows gets a std of exactly 0. */
+#define ZEGGS_MOMENTS_MAX_GROUPS 8
+typedef struct {
+  int n_groups;
+  const float* src[ZEGGS_MOMENTS_MAX_GROUPS];
+  int width[ZEGGS_MOMENTS_MAX_GROUPS];
+  const int* rows;
+  long long n_sel;
+  double *mean, *std, *group_std;
+  void* workspace;
+  size_t workspace_bytes;
+} zeggs_moments_args;
+size_t zeggs_masked_moments_workspace_bytes(long long n_sel, int total_width);
+int zeggs_masked_moments(const zeggs_moments_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -99,6 +99,19 @@ LossArgs = _struct("LossArgs", ints=("B", "T", "Z"), floats=("dt", "kl_weight"),
                          "losses", "dY", "dRootPos", "dRootRot", "dmu", "dlogvar", "workspace"),
                    tail=[("workspace_bytes", C.c_size_t), ("kl_weight_dev", C.c_void_p)])
 
+AnimFeaturesArgs = _struct("AnimFeaturesArgs", ints=("T", "J"),
+                           tail=[("order", C.c_int * 3), ("spine2", C.c_int), ("hips", C.c_int), ("head", C.c_int), ("dt", C.c_double)] +
+                           [(n, C.c_void_p) for n in ("rotations", "positions", "parents", "root_pos", "root_rot", "root_vel", "root_vrt",
+                                                      "lpos", "ltxy", "lvel", "lvrt", "gaze_pos", "gaze_dir", "quat_out", "workspace")] +
+                           [("workspace_bytes", C.c_size_t)])
+SplineArgs = _struct("SplineArgs", tail=[("n", C.c_longlong), ("m", C.c_longlong), ("C", C.c_int), ("in_f64", C.c_int), ("x", C.c_void_p),
+                                         ("y", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
+MOMENTS_MAX_GROUPS = 8
+MomentsArgs = _struct("MomentsArgs", ints=("n_groups",),
+                      tail=[("src", C.c_void_p * MOMENTS_MAX_GROUPS), ("width", C.c_int * MOMENTS_MAX_GROUPS), ("rows", C.c_void_p),
+                            ("n_sel", C.c_longlong), ("mean", C.c_void_p), ("std", C.c_void_p), ("group_std", C.c_void_p),
+                            ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
+
 
 # every symbol include/zeggs_b200.h declares: (name, restype, argtypes)
 # C struct name -> ctypes mirror (checked against the library's sizeof at test time: tests/test_abi_cpu.py)
@@ -107,7 +120,8 @@ def struct_mirrors():
             "zeggs_decoder_bwd_args": DecoderBwdArgs, "zeggs_speech_enc_args": SpeechEncArgs, "zeggs_speech_enc_grads": SpeechEncGrads,
             "zeggs_style_enc_args": StyleEncArgs, "zeggs_style_enc_grads": StyleEncGrads, "zeggs_decoder_step_args": DecoderStepArgs,
             "zeggs_loss_args": LossArgs, "zeggs_pose_post_args": PosePostArgs, "zeggs_gather_args": GatherArgs,
-            "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads}
+            "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads,
+            "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs}
 
 
 SYMBOLS = [
@@ -166,6 +180,13 @@ SYMBOLS = [
     ("zeggs_gemm_f32_ctx", C.c_int, [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_int, C.c_int, C.c_void_p]),
     ("zeggs_split_bf16", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    ("zeggs_anim_features_workspace_bytes", C.c_size_t, [C.c_int, C.c_int]),
+    ("zeggs_anim_features", C.c_int, [C.POINTER(AnimFeaturesArgs), C.c_void_p]),
+    ("zeggs_quat_to_euler_deg", C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
+    ("zeggs_spline_resample_workspace_bytes", C.c_size_t, [C.c_longlong, C.c_int]),
+    ("zeggs_spline_resample", C.c_int, [C.POINTER(SplineArgs), C.c_void_p]),
+    ("zeggs_masked_moments_workspace_bytes", C.c_size_t, [C.c_longlong, C.c_int]),
+    ("zeggs_masked_moments", C.c_int, [C.POINTER(MomentsArgs), C.c_void_p]),
 ]
 
 _lib = None

@@ -17,15 +17,16 @@ def _walk(parents):
     return children
 
 
-def save_bvh(filename, positions, rotations_deg, parents, names=None, order="zyx", frametime=1.0 / 60.0):
-    """positions [T,J,3] (joint 0 = root trajectory; the first frame gives every OFFSET), rotations_deg [T,J,3] in `order`."""
+def save_bvh(filename, positions, rotations_deg, parents, names=None, order="zyx", frametime=1.0 / 60.0, offsets=None):
+    """positions [T,J,3] (joint 0 = root trajectory), rotations_deg [T,J,3] in `order`; offsets [J,3] gives every OFFSET (default: the
+    first frame of positions)."""
     positions = np.asarray(positions)
     rotations_deg = np.asarray(rotations_deg)
     parents = [int(p) for p in parents]
     J = len(parents)
     names = list(names) if names is not None else [f"joint_{i}" for i in range(J)]
     children = _walk(parents)
-    offsets = positions[0]
+    offsets = positions[0] if offsets is None else np.asarray(offsets)
     rot_names = " ".join(_CH[c] for c in order)
     lines, seq = [], []
 

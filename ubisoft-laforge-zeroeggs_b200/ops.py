@@ -755,3 +755,114 @@ def decoder_step(dec, pose, speech, style, state):
         setattr(a, n, t.data_ptr())
     _lib.check(l.zeggs_decoder_step_fwd(a, _lib.stream_ptr()), "zeggs_decoder_step_fwd")
     return y, h_out
+
+
+# ---------------------------------------------------------------------------------------------- training-set construction
+_EULER_AXIS = {"x": 0, "y": 1, "z": 2}
+_TO_EULER = {"zyx": 0, "xzy": 1}
+
+
+def _f64c(t, device):
+    return torch.as_tensor(t).to(device=device, dtype=torch.float64).contiguous()
+
+
+def anim_features(rotations, positions, parents, order, dt, spine2, hips, head, device="cuda"):
+    """data_pipeline.py:90-228 on the device for one take: rotations [T,J,3] (degrees, BVH channel order `order`), positions [T,J,3],
+    parents [J] -> dict of float32 CUDA tensors root_pos, root_rot, root_vel, root_vrt, lpos, ltxy, lvel, lvrt, gaze_pos, gaze_dir
+    with the reference's shapes.  The arithmetic is float64."""
+    dev = torch.device(device)
+    rot, pos = _f64c(rotations, dev), _f64c(positions, dev)
+    T, J = int(rot.shape[0]), int(rot.shape[1])
+    par = torch.as_tensor(parents, dtype=torch.int32).to(dev).contiguous()
+    shapes = dict(root_pos=(T, 3), root_rot=(T, 4), root_vel=(T, 3), root_vrt=(T, 3), lpos=(T, J, 3), ltxy=(T, J, 2, 3), lvel=(T, J, 3),
+                  lvrt=(T, J, 3), gaze_pos=(T, 3), gaze_dir=(T, 3))
+    out = {k: torch.empty(s, dtype=torch.float32, device=dev) for k, s in shapes.items()}
+    _anim_call(rot, pos, par, order, dt, (spine2, hips, head), out, None)
+    return out
+
+
+def unrolled_quaternions(rotations, parents, order, device="cuda"):
+    """quat.unroll(quat.from_euler(radians(rotations), order)) on the device: [T,J,3] degrees -> [T,J,4] float64 CUDA tensor."""
+    dev = torch.device(device)
+    rot = _f64c(rotations, dev)
+    par = torch.as_tensor(parents, dtype=torch.int32).to(dev).contiguous()
+    q = torch.empty((rot.shape[0], rot.shape[1], 4), dtype=torch.float64, device=dev)
+    _anim_call(rot, None, par, order, 1.0, (0, 0, 0), None, q)
+    return q
+
+
+def _anim_call(rot, pos, par, order, dt, joints, out, quat_out):
+    l = _lib.lib()
+    T, J = int(rot.shape[0]), int(rot.shape[1])
+    if rot.shape[2:] != (3,) or (pos is not None and tuple(pos.shape) != (T, J, 3)) or par.numel() != J:
+        raise _lib.ZeggsError(f"anim_features: rotations {tuple(rot.shape)}, positions {None if pos is None else tuple(pos.shape)}, "
+                              f"{par.numel()} parents")
+    if len(order) != 3 or any(c not in _EULER_AXIS for c in order):
+        raise _lib.ZeggsError(f"anim_features: Euler order {order!r}")
+    wsb = l.zeggs_anim_features_workspace_bytes(T, J)
+    ws = WS.get("anim_features", max(wsb, 1), rot.device)
+    a = _lib.AnimFeaturesArgs(T=T, J=J, spine2=int(joints[0]), hips=int(joints[1]), head=int(joints[2]), dt=float(dt),
+                              rotations=rot.data_ptr(), positions=pos.data_ptr() if pos is not None else None, parents=par.data_ptr(),
+                              quat_out=quat_out.data_ptr() if quat_out is not None else None, workspace=ws.data_ptr(), workspace_bytes=wsb)
+    for i, c in enumerate(order):
+        a.order[i] = _EULER_AXIS[c]
+    if out is not None:
+        for k, t in out.items():
+            setattr(a, k, t.data_ptr())
+    _lib.check(l.zeggs_anim_features(a, _lib.stream_ptr()), "zeggs_anim_features")
+
+
+def quat_to_euler_deg(q, order):
+    """quat.normalize -> quat.to_euler(order) -> np.degrees on the device: [..., 4] float64 CUDA -> [..., 3] float64."""
+    if order not in _TO_EULER:
+        raise _lib.ZeggsError(f"to_euler converts to 'zyx' or 'xzy' only, not {order!r} (the reference raises NotImplementedError)")
+    q = q.to(torch.float64).contiguous()
+    e = torch.empty(q.shape[:-1] + (3,), dtype=torch.float64, device=q.device)
+    _lib.check(_lib.lib().zeggs_quat_to_euler_deg(_lib.ptr(q), _lib.ptr(e), q.numel() // 4, _TO_EULER[order], _lib.stream_ptr()),
+               "zeggs_quat_to_euler_deg")
+    return e
+
+
+def spline_resample(x, m):
+    """griddata(arange(n), x, linspace(0, n-1, m), method="cubic") along dim 0 (data_pipeline.py:415-432): x [n] or [n, ...] float32 /
+    float64 CUDA tensor -> [m] or [m, ...] float64."""
+    if not x.is_cuda:
+        raise _lib.ZeggsError("spline_resample runs on CUDA tensors only (no CPU fallback)")
+    if x.dtype not in (torch.float32, torch.float64):
+        x = x.to(torch.float64)
+    x = x.contiguous()
+    n = int(x.shape[0])
+    C = int(x[0].numel()) if n else 1
+    l = _lib.lib()
+    y = torch.empty((int(m),) + tuple(x.shape[1:]), dtype=torch.float64, device=x.device)
+    wsb = l.zeggs_spline_resample_workspace_bytes(n, C)
+    ws = WS.get("spline", max(wsb, 1), x.device)
+    a = _lib.SplineArgs(n=n, m=int(m), C=C, in_f64=int(x.dtype == torch.float64), x=x.data_ptr(), y=y.data_ptr(), workspace=ws.data_ptr(),
+                        workspace_bytes=wsb)
+    _lib.check(l.zeggs_spline_resample(a, _lib.stream_ptr()), "zeggs_spline_resample")
+    return y
+
+
+def masked_moments(groups, rows):
+    """Per-channel mean and population std, and the pooled population std of each group, over the rows `rows` (data_pipeline.py:562-648).
+    groups: list of float32 CUDA tensors [n_rows, ...] (flattened per row); rows: int index tensor.  -> (mean [sum widths] f64,
+    std [sum widths] f64, group_std [len(groups)] f64), CUDA tensors."""
+    if not 1 <= len(groups) <= _lib.MOMENTS_MAX_GROUPS:
+        raise _lib.ZeggsError(f"masked_moments: {len(groups)} groups (1..{_lib.MOMENTS_MAX_GROUPS})")
+    dev = groups[0].device
+    srcs = [g.reshape(g.shape[0], -1).to(torch.float32).contiguous() for g in groups]
+    rows = torch.as_tensor(rows, dtype=torch.int32).to(dev).contiguous()
+    W = sum(int(s.shape[1]) for s in srcs)
+    mean = torch.empty(W, dtype=torch.float64, device=dev)
+    std = torch.empty(W, dtype=torch.float64, device=dev)
+    gstd = torch.empty(len(srcs), dtype=torch.float64, device=dev)
+    l = _lib.lib()
+    wsb = l.zeggs_masked_moments_workspace_bytes(int(rows.numel()), W)
+    ws = WS.get("moments", max(wsb, 1), dev)
+    a = _lib.MomentsArgs(n_groups=len(srcs), rows=_lib.ptr(rows), n_sel=int(rows.numel()), mean=mean.data_ptr(), std=std.data_ptr(),
+                         group_std=gstd.data_ptr(), workspace=ws.data_ptr(), workspace_bytes=wsb)
+    for i, s in enumerate(srcs):
+        a.src[i] = _lib.ptr(s)
+        a.width[i] = int(s.shape[1])
+    _lib.check(l.zeggs_masked_moments(a, _lib.stream_ptr()), "zeggs_masked_moments")
+    return mean, std, gstd
