@@ -485,6 +485,31 @@ typedef struct {
 size_t zeggs_masked_moments_workspace_bytes(long long n_sel, int total_width);
 int zeggs_masked_moments(const zeggs_moments_args* a, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Rate conversion of a WAV file's samples to 16 kHz mono.  Replaces the SoX step of the reference's read_wavfile
+ * (audio/audio_files.py:52-78 reformat_and_trim_wav_file: `rate -h`, `channels 1`, 32-bit output; :88-163 read_wavfile), which
+ * generate.py:161-170 reaches for any file that is not 16 kHz.  One launch: decode the interleaved PCM pcm [n_in, channels]
+ * (int16 x/2^15, int32 x/2^31, uint8 (u-128)/128, float32 clipped to [-1, 1]), average the channels, polyphase FIR, clamp the
+ * result to [-1, 1] -> out [n_out] f32.  The rate ratio is L/M in lowest terms (L <= 1024).  taps [L, K4] f32 (16-byte aligned,
+ * K4 % 4 == 0): taps[p][q] = h[p + q L] of a prototype h at rate L * fs_in whose centre tap is h[delay]; output j is
+ *   sum_q taps[p][q] * x[(j M + delay) / L - q],  p = (j M + delay) mod L,  x = 0 outside [0, n_in)
+ * (zeggs_b200.audio.design_resampler builds the prototype; n_out = floor(n_in * L / M + 1/2) is what SoX's rate effect emits).
+ * ZEGGS_ERR_UNSUPPORTED when the input span of one CTA does not fit in shared memory (L/M far beyond 192 kHz -> 16 kHz). */
+#define ZEGGS_PCM_I16 0
+#define ZEGGS_PCM_I32 1
+#define ZEGGS_PCM_U8 2
+#define ZEGGS_PCM_F32 3
+typedef struct {
+  long long n_in, n_out;
+  int channels, dtype;    /* dtype: ZEGGS_PCM_* */
+  int L, M, K4;
+  long long delay;
+  const void* pcm;
+  const float* taps;
+  float* out;
+} zeggs_resample_args;
+int zeggs_resample(const zeggs_resample_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -111,6 +111,9 @@ MomentsArgs = _struct("MomentsArgs", ints=("n_groups",),
                       tail=[("src", C.c_void_p * MOMENTS_MAX_GROUPS), ("width", C.c_int * MOMENTS_MAX_GROUPS), ("rows", C.c_void_p),
                             ("n_sel", C.c_longlong), ("mean", C.c_void_p), ("std", C.c_void_p), ("group_std", C.c_void_p),
                             ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
+ResampleArgs = _struct("ResampleArgs", tail=[("n_in", C.c_longlong), ("n_out", C.c_longlong), ("channels", C.c_int), ("dtype", C.c_int),
+                                             ("L", C.c_int), ("M", C.c_int), ("K4", C.c_int), ("delay", C.c_longlong), ("pcm", C.c_void_p),
+                                             ("taps", C.c_void_p), ("out", C.c_void_p)])
 
 
 # every symbol include/zeggs_b200.h declares: (name, restype, argtypes)
@@ -121,7 +124,8 @@ def struct_mirrors():
             "zeggs_style_enc_args": StyleEncArgs, "zeggs_style_enc_grads": StyleEncGrads, "zeggs_decoder_step_args": DecoderStepArgs,
             "zeggs_loss_args": LossArgs, "zeggs_pose_post_args": PosePostArgs, "zeggs_gather_args": GatherArgs,
             "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads,
-            "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs}
+            "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs,
+            "zeggs_resample_args": ResampleArgs}
 
 
 SYMBOLS = [
@@ -187,6 +191,7 @@ SYMBOLS = [
     ("zeggs_spline_resample", C.c_int, [C.POINTER(SplineArgs), C.c_void_p]),
     ("zeggs_masked_moments_workspace_bytes", C.c_size_t, [C.c_longlong, C.c_int]),
     ("zeggs_masked_moments", C.c_int, [C.POINTER(MomentsArgs), C.c_void_p]),
+    ("zeggs_resample", C.c_int, [C.POINTER(ResampleArgs), C.c_void_p]),
 ]
 
 _lib = None

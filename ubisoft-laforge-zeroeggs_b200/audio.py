@@ -175,8 +175,109 @@ class LoudnessMeter:
         return (gain, lufs) if want_lufs else gain
 
 
+RESAMPLE_ATTEN_DB = 125.5        # Kaiser design attenuation: the measured stopband then stays below -124 dB in fp32 at every rate
+RESAMPLE_MAX_L = 1024
+PCM_DTYPES = {np.dtype(np.int16): 0, np.dtype(np.int32): 1, np.dtype(np.uint8): 2, np.dtype(np.float32): 3}   # zeggs_resample_args.dtype
+
+
+def resample_ratio(fs_in, fs_out=16000):
+    """(L, M) with L / M = fs_out / fs_in in lowest terms; a ZeggsError names the rate when L > RESAMPLE_MAX_L."""
+    fs_in, fs_out = int(fs_in), int(fs_out)
+    if fs_in <= 0 or fs_out <= 0:
+        raise _lib.ZeggsError(f"cannot resample {fs_in} Hz audio to {fs_out} Hz")
+    g = math.gcd(fs_in, fs_out)
+    L, M = fs_out // g, fs_in // g
+    if L > RESAMPLE_MAX_L:
+        raise _lib.ZeggsError(f"cannot resample {fs_in} Hz audio to {fs_out} Hz: the rate ratio reduces to {L}/{M} and the "
+                              f"polyphase filter supports at most {RESAMPLE_MAX_L} phases")
+    return L, M
+
+
+def resampled_length(n_in, fs_in, fs_out=16000):
+    """floor(n_in * fs_out / fs_in + 0.5) in exact integers: the length SoX's rate effect flushes (samples_in / factor + .5)."""
+    return (2 * int(n_in) * int(fs_out) + int(fs_in)) // (2 * int(fs_in))
+
+
+def design_resampler(fs_in, fs_out=16000, atten_db=RESAMPLE_ATTEN_DB):
+    """Linear-phase Kaiser-windowed sinc prototype at rate L * fs_in, float64, gain L (SoX `rate -h` parameters: passband to
+    0.95 f_N, stopband from f_N = min(fs_in, fs_out) / 2, ~125 dB rejection).  Length from the Kaiser formula, rounded up to a
+    multiple of L and made odd, so the filter is symmetric about its centre tap (n - 1) / 2.  Returns (h, L, M)."""
+    L, M = resample_ratio(fs_in, fs_out)
+    F = float(L * int(fs_in))
+    f_n = min(int(fs_in), int(fs_out)) / 2.0
+    f_pass, f_stop = 0.95 * f_n, f_n
+    fc = 0.5 * (f_pass + f_stop)
+    dw = 2.0 * np.pi * (f_stop - f_pass) / F
+    n = int(math.ceil((atten_db - 7.95) / (2.285 * dw))) + 1
+    n = -(-n // L) * L
+    n += 1 - n % 2
+    beta = 0.1102 * (atten_db - 8.7)
+    k = np.arange(n, dtype=np.float64) - (n - 1) / 2.0
+    h = L * (2.0 * fc / F) * np.sinc((2.0 * fc / F) * k) * np.kaiser(n, beta)
+    return h, L, M
+
+
+def polyphase_table(h, L):
+    """Prototype h -> fp32 table [L, K4] with table[p, q] = h[p + q L] (zero past the end), K4 = ceil(len(h) / L) rounded up to 4."""
+    K = -(-len(h) // L)
+    K4 = -(-K // 4) * 4
+    hp = np.zeros(L * K4, dtype=np.float64)
+    hp[:len(h)] = h
+    return np.ascontiguousarray(hp.reshape(K4, L).T.astype(np.float32)), K
+
+
+class Resampler:
+    """Rate conversion of raw WAV PCM to fs_out (zeggs_resample): decode as SoX does, average the channels, polyphase FIR with
+    the design_resampler prototype, clamp to [-1, 1].  The polyphase table is built on the host in float64 and kept on the device."""
+
+    def __init__(self, device, fs_in, fs_out=16000):
+        self.device = torch.device(device)
+        self.fs_in, self.fs_out = int(fs_in), int(fs_out)
+        self.h, self.L, self.M = design_resampler(fs_in, fs_out)
+        self.delay = (len(self.h) - 1) // 2
+        table, self.K = polyphase_table(self.h, self.L)
+        self.table = torch.from_numpy(table).to(self.device)
+
+    def __call__(self, pcm):
+        """pcm [n] or [n, C] (numpy or torch; int16, int32, uint8, float32 or float64) -> float32 [n_out] on the device."""
+        if isinstance(pcm, np.ndarray):
+            x = pcm.astype(np.float32) if pcm.dtype == np.float64 else pcm
+            if x.dtype not in PCM_DTYPES:
+                raise _lib.ZeggsError(f"unsupported PCM sample type {x.dtype}")
+            x = torch.from_numpy(np.ascontiguousarray(x))
+        else:
+            x = pcm.float() if pcm.dtype == torch.float64 else pcm
+        code = {torch.int16: 0, torch.int32: 1, torch.uint8: 2, torch.float32: 3}.get(x.dtype)
+        if code is None:
+            raise _lib.ZeggsError(f"unsupported PCM sample type {x.dtype}")
+        if x.dim() == 1:
+            x = x[:, None]
+        if x.dim() != 2 or x.shape[1] < 1:
+            raise _lib.ZeggsError(f"PCM must be [n_samples] or [n_samples, channels], got {tuple(x.shape)}")
+        if not x.is_cuda:
+            x = x.contiguous().pin_memory().to(self.device, non_blocking=True)
+        x = x.contiguous()
+        n_in, C = x.shape
+        n_out = resampled_length(n_in, self.fs_in, self.fs_out)
+        out = torch.empty(n_out, dtype=torch.float32, device=x.device)
+        a = _lib.ResampleArgs(n_in=n_in, n_out=n_out, channels=C, dtype=code, L=self.L, M=self.M, K4=int(self.table.shape[1]),
+                              delay=self.delay, pcm=_lib.ptr(x), taps=_lib.ptr(self.table), out=_lib.ptr(out))
+        _lib.check(_lib.lib().zeggs_resample(a, _lib.stream_ptr()), "zeggs_resample")
+        return out
+
+
 _cache = {}
 _meters = {}
+_resamplers = {}
+
+
+def resample(pcm, fs_in, fs_out=16000, device="cuda"):
+    """Raw WAV PCM at fs_in ([n] or [n, C], as scipy.io.wavfile.read returns it) -> float32 [n_out] CUDA tensor at fs_out: what
+    the reference's read_wavfile(..., desired_fs=16000) gets back from SoX (audio_files.py:52-78, 115-146)."""
+    key = (str(torch.device(device)), int(fs_in), int(fs_out))
+    if key not in _resamplers:
+        _resamplers[key] = Resampler(device, fs_in, fs_out)
+    return _resamplers[key](pcm)
 
 
 def _meter(device, rate):

@@ -40,7 +40,10 @@ def read_wav(path):
     """scipy read + the reference's int->float rescale (audio_files.py:211-236); 16 kHz mono expected (generate.py:161-168).
     16-bit PCM is returned as int16 (the rescale x / 32768 happens on the device), everything else as float32."""
     from scipy.io import wavfile
-    fs, x = wavfile.read(str(path))
+    return _decode_16k(path, *wavfile.read(str(path)))
+
+
+def _decode_16k(path, fs, x):
     if x.ndim > 1:
         x = x[:, 0]
     if fs != 16000:
@@ -137,10 +140,15 @@ def generate_gesture(audio_file, styles, network_path, data_path, results_path, 
     with torch.no_grad():
         speech = None
         if audio_file is not None:
-            wav = read_wav(audio_file)                                                    # int16 PCM stays int16: decoded on the device
+            from scipy.io import wavfile
+            fs, pcm = wavfile.read(str(audio_file))
+            if fs == 16000:
+                wav = torch.from_numpy(_decode_16k(audio_file, fs, pcm))                 # int16 PCM stays int16: decoded on the device
+            else:
+                wav = audio.resample(pcm, fs, 16000, device=device)                       # what SoX hands back (audio_files.py:115-146)
             n_frames = int(round(60.0 * (len(wav) / 16000)))                              # generate.py:170
             ac = conf["audio_conf"] if "audio_conf" in conf else conf
-            feats = audio.preprocess_audio(torch.from_numpy(wav), 60, n_frames, ac, conf.get("audio_feature_type", ["mel_spec", "energy"]), device=device)
+            feats = audio.preprocess_audio(wav, 60, n_frames, ac, conf.get("audio_feature_type", ["mel_spec", "energy"]), device=device)
             speech = nets["speech_encoder"]((feats[None] - f("audio_input_mean")) / f("audio_input_std"))
         for style in styles:
             if style_encoding_type == "example":
