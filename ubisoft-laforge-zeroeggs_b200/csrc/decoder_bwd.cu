@@ -481,6 +481,158 @@ static int rowsum(const float* GA, long long gaT, long long gaBT, int N, int nT,
   return ZEGGS_OK;
 }
 
+WgradHists wgrad_hists(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
+                       const BwdWs& bw, bool want_lo) {
+  const int H = a.H, nbt = g.nbt, C = a.S + a.Z;
+  const long long sH = (long long)nbt * H * 32, s3 = (long long)nbt * 3 * H * 32, sX = (long long)nbt * K1P * 32, sC = (long long)nbt * C * 32;
+  WgradHists hs = {{
+      {bw.DY, sX, P_OUT, nullptr, nullptr, b.db2}, {bw.DGI1, s3, 3 * H, nullptr, nullptr, b.db_ih1}, {bw.DGH1, s3, 3 * H, nullptr, nullptr, b.db_hh1},
+      {bw.DGI0, s3, 3 * H, nullptr, nullptr, b.db_ih0}, {bw.DGH0, s3, 3 * H, nullptr, nullptr, b.db_hh0}, {bw.DPA, sH, H, nullptr, nullptr, b.db0},
+      {w.H0, sH, H, nullptr, nullptr, nullptr}, {w.H1, sH, H, nullptr, nullptr, nullptr}, {w.A, sH, H, nullptr, nullptr, nullptr},
+      {w.XP, sX, P_IN, nullptr, nullptr, nullptr}, {bw.COND, sC, C, nullptr, nullptr, nullptr}}};
+  hs.slots = a.T * nbt;
+  hs.nbt = nbt;
+  hs.ld = (size_t)hs.slots * 32;
+  char* base = scratch_base();
+  size_t off = 0;
+  auto take = [&](int rows) {
+    __nv_bfloat16* p = base ? (__nv_bfloat16*)(base + off) : nullptr;
+    off += (size_t)rows * hs.ld * 2;
+    return p;
+  };
+  for (auto& h : hs.h) h.hi = take(h.rows);
+  if (want_lo) for (auto& h : hs.h) h.lo = take(h.rows);
+  hs.bytes = off;
+  hs.end = base ? base + off : nullptr;
+  return hs;
+}
+
+int split_hist(const WgradHists& hs, int i, cudaStream_t stream) {
+  // per-slot stride of the fp32 history is (stride / nbt) floats: slots (t,bt) are contiguous.  The bias gradient is the sum over
+  // slots t >= 1, i.e. s >= nbt
+  const WgradHist& h = hs.h[i];
+  return split_hist_launch(h.src, h.stride / hs.nbt, hs.slots, h.rows, h.hi, h.lo, stream, h.db, hs.nbt);
+}
+
+int wgrad_gemms(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const WgradHists& hs, bool want_lo,
+                char* tail, cudaStream_t stream) {
+  const int H = a.H, A = g.A, C = a.S + a.Z;
+  const int cur = g.nbt * 32;                       // column offset of slot t = 1
+  const int Kc = (a.T - 1) * g.nbt * 32;
+  char* ws_p = (char*)(((uintptr_t)tail + 255) & ~(uintptr_t)255);
+  const size_t ws_bytes = (size_t)(scratch_base() + scratch_bytes() - ws_p);
+  auto G = [&](int ga, int ga_off, int N, int xb, int xb_off, int K, float* dW, int ldw) {
+    const WgradHist &x = hs.h[ga], &y = hs.h[xb];
+    return tc_gemm_launch(N, K, Kc, x.hi + ga_off, want_lo ? x.lo + ga_off : nullptr, (int)hs.ld,
+                          y.hi + xb_off, want_lo ? y.lo + xb_off : nullptr, (int)hs.ld, nullptr, dW, ldw, 0, 0, stream,
+                          (float*)ws_p, ws_bytes);
+  };
+  int rc;
+  if ((rc = G(HDY, cur, P_OUT, HH1, cur, H, b.dW2, H))) return rc;
+  if ((rc = G(HGI1, cur, 3 * H, HH0, cur, H, b.dW_ih1, H))) return rc;
+  if ((rc = G(HGH1, cur, 3 * H, HH1, 0, H, b.dW_hh1, H))) return rc;
+  if ((rc = G(HGI0, cur, 3 * H, HA, cur, H + P_IN + C, b.dW_ih0, A + H))) return rc;     // [a | x_pose | cond] stacked
+  if ((rc = G(HGH0, cur, 3 * H, HH0, 0, H, b.dW_hh0, H))) return rc;
+  return G(HPA, cur, H, HXP, cur, P_IN + C, b.dW0, A);                                    // [x_pose | cond] stacked
+}
+
+int cond_kmajor(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdWs& bw, cudaStream_t stream) {
+  cond_kmajor_kernel<<<592, 256, 0, stream>>>(a, g, bw.COND);
+  count_launch();
+  ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+int cse_backward(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecWs& w, const BwdWs& bw, cudaStream_t stream) {
+  const int H = a.H, Kin = P_IN + a.Z;
+  int r;
+  cse_gather_kernel<<<ceil_div(a.B * 2 * H, 256), 256, 0, stream>>>(a.B, H, bw.DH0, bw.DH1, bw.cse_dout);
+  count_launch();
+  r = sgemm_launch(1, 2 * H, H, a.B, bw.cse_dout, 2 * H, w.cse_h2, H, nullptr, b.dWc2, H, 0, 0, stream); if (r) return r;
+  colsum_kernel<<<ceil_div(2 * H, 256), 256, 0, stream>>>(bw.cse_dout, a.B, 2 * H, b.dbc2); count_launch();
+  r = gemm_f32_auto(2, a.B, H, 2 * H, bw.cse_dout, 2 * H, a.Wc2, H, nullptr, bw.cse_d2, H, 0, 0, stream); if (r) return r;
+  elu_bwd_kernel<<<ceil_div(a.B * H, 256), 256, 0, stream>>>(bw.cse_d2, w.cse_h2, (size_t)a.B * H); count_launch();
+  r = sgemm_launch(1, H, H, a.B, bw.cse_d2, H, w.cse_h1, H, nullptr, b.dWc1, H, 0, 0, stream); if (r) return r;
+  colsum_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d2, a.B, H, b.dbc1); count_launch();
+  r = gemm_f32_auto(2, a.B, H, H, bw.cse_d2, H, a.Wc1, H, nullptr, bw.cse_d1, H, 0, 0, stream); if (r) return r;
+  elu_bwd_kernel<<<ceil_div(a.B * H, 256), 256, 0, stream>>>(bw.cse_d1, w.cse_h1, (size_t)a.B * H); count_launch();
+  r = sgemm_launch(1, H, Kin, a.B, bw.cse_d1, H, w.cse_in, Kin, nullptr, b.dWc0, Kin, 0, 0, stream); if (r) return r;
+  colsum_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d1, a.B, H, b.dbc0); count_launch();
+  r = gemm_f32_auto(2, a.B, Kin, H, bw.cse_d1, H, a.Wc0, Kin, nullptr, bw.cse_din, Kin, 0, 0, stream); if (r) return r;
+  ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+int dy_combine(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const float* dxp, const BwdWs& bw, cudaStream_t stream) {
+  dy_combine_kernel<<<dim3(a.T - 1, ceil_div(P_OUT, 64)), 256, 0, stream>>>(a, b.dY, dxp, bw.DCH, bw.DY);
+  count_launch();
+  ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+int dcond_scatter(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const BwdWs& bw, int rows,
+                  cudaStream_t stream) {
+  dcond_scatter_kernel<<<592, 256, 0, stream>>>(a, g, bw.DCOND, bw.cse_din, b.dSpeech, b.dStyle, rows);
+  count_launch();
+  ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+// fp32 engine: the SIMT BPTT recurrence, then the weight gradients, d cond, the CellStateEncoder backward and the dSpeech / dStyle
+// scatter.  It does all of it in phase 1 (or 0) and nothing in phase 2.
+static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
+                                   const BwdWs& bw, cudaStream_t stream) {
+  ZCHECK_ARG(b.packed_bwd, "decoder bwd: packed_bwd missing");
+  if (b.phase == 2) return ZEGGS_OK;
+  const int H = a.H, T = a.T, nbt = g.nbt, C = a.S + a.Z, A = g.A, nT = T - 1;
+  int rc;
+  ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
+  ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
+  {
+    const BwdGeom bg = make_bgeom(g);
+    BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
+    ScopedTimer tm("decoder_bwd", stream);
+    rc = g.U == 4 ? launch_bwd<4>(a, g, bg, w, bw, d, stream) : launch_bwd<8>(a, g, bg, w, bw, d, stream);
+    if (rc) return rc;
+  }
+  ScopedTimer tm("decoder_wgrad", stream);
+  if ((rc = cond_kmajor(a, g, bw, stream))) return rc;
+  const long long sH = (long long)nbt * H * 32, s3 = (long long)nbt * 3 * H * 32, sX = (long long)nbt * K1P * 32, sC = (long long)nbt * C * 32;
+  // weight gradients: tensor-core GEMMs over split-bf16 copies of the histories when those fit the scratch buffer (a second, lo pass
+  // in GEMM mode 1 for ~fp32 accuracy), the SIMT k-major kernels otherwise
+  const bool want_lo = gemm_mode() == 1;
+  const WgradHists hs = wgrad_hists(a, b, g, w, bw, want_lo);
+  if (gemm_mode() != 0 && scratch_base() != nullptr && hs.bytes <= scratch_bytes()) {
+    for (int i = 0; i < NHIST; ++i) if ((rc = split_hist(hs, i, stream))) return rc;
+    if ((rc = wgrad_gemms(a, b, g, hs, want_lo, hs.end, stream))) return rc;
+  } else {
+    // layer2: dW2 = DY . H1[t]^T
+    if ((rc = wgrad(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, w.H1 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW2, H, stream))) return rc;
+    if ((rc = rowsum(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, nT, nbt, b.db2, stream))) return rc;
+    // GRU layer 1
+    if ((rc = wgrad(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih1, H, stream))) return rc;
+    if ((rc = wgrad(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H1, sH, (long long)H * 32, H, nT, nbt, b.dW_hh1, H, stream))) return rc;
+    if ((rc = rowsum(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih1, stream))) return rc;
+    if ((rc = rowsum(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh1, stream))) return rc;
+    // GRU layer 0: input = [a | x_pose | cond]
+    if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.A + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih0, A + H, stream))) return rc;
+    if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW_ih0 + H, A + H, stream))) return rc;
+    if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW_ih0 + H + P_IN, A + H, stream))) return rc;
+    if ((rc = wgrad(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0, sH, (long long)H * 32, H, nT, nbt, b.dW_hh0, H, stream))) return rc;
+    if ((rc = rowsum(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih0, stream))) return rc;
+    if ((rc = rowsum(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh0, stream))) return rc;
+    // layer0
+    if ((rc = wgrad(bw.DPA + sH, sH, (long long)H * 32, H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW0, A, stream))) return rc;
+    if ((rc = wgrad(bw.DPA + sH, sH, (long long)H * 32, H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW0 + P_IN, A, stream))) return rc;
+    if ((rc = rowsum(bw.DPA + sH, sH, (long long)H * 32, H, nT, nbt, b.db0, stream))) return rc;
+  }
+  // d cond[t] = W0[:, 1134:]^T dpre_a + W_ih0[:, H+1134:]^T dgi0   (batched over slots t >= 1)
+  rc = sgemm_batched_launch(1, C, 32, H, a.W0 + P_IN, A, bw.DPA + sH, 32, nullptr, bw.DCOND + sC, 32, 0, 0, nT * nbt, 0, (long long)H * 32, (long long)C * 32, stream); if (rc) return rc;
+  rc = sgemm_batched_launch(1, C, 32, 3 * H, a.W_ih0 + H + P_IN, A + H, bw.DGI0 + s3, 32, nullptr, bw.DCOND + sC, 32, 0, 1, nT * nbt, 0, (long long)3 * H * 32, (long long)C * 32, stream); if (rc) return rc;
+  if ((rc = cse_backward(a, b, w, bw, stream))) return rc;
+  return dcond_scatter(a, b, g, bw, 0, stream);
+}
+
 extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const zeggs_decoder_bwd_args* bp, void* stream_) {
   CtxScope ctx_scope(ap ? ap->ctx : nullptr);
   ZCHECK_ARG(ap && bp, "decoder bwd: null args");
@@ -504,197 +656,12 @@ extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const 
     return ZEGGS_OK;
   }
   DecGeom g = make_geom(a.B, a.H, a.S, a.Z);
-  BwdGeom bg = make_bgeom(g);
   DecWs w = make_ws(a.workspace, g, a.T, 1);
   BwdWs bw = make_bws(b.workspace, g, a.T);
   ZCHECK_ARG(b.workspace && b.workspace_bytes >= bw.bytes, "decoder bwd: workspace too small (%zu < %zu)", b.workspace_bytes, bw.bytes);
-  const bool use_tc = a.engine == 1 && b.packed_bwd_tc != nullptr && g.nbt == 1 && bg.n4b == 1;
-  ZCHECK_ARG(use_tc || b.packed_bwd, "decoder bwd: packed_bwd missing");
-  const int H = a.H, T = a.T, nbt = g.nbt, C = a.S + a.Z, A = g.A;
-  // phase 0: the whole backward.  The tensor-core engine can run it in two calls so that the encoders' backward passes (which need only
-  // dSpeech / dStyle) overlap the large weight-gradient GEMMs on other streams: phase 1 = BPTT recurrence + CellStateEncoder backward +
-  // the conditioning gradients (dSpeech, dStyle); phase 2 = every remaining parameter gradient.  Other engines do all of it in phase 1.
-  const int phase = b.phase;
-  ZCHECK_ARG(phase >= 0 && phase <= 2, "decoder bwd: phase must be 0, 1 or 2");
-  const bool fold = use_tc && nbt == 1 && H % 64 == 0 && gemm_mode() != 0 && scratch_base() != nullptr;
-  const bool p1 = phase != 2, p2 = phase != 1 || !fold;
-  if (phase == 2 && !fold) return ZEGGS_OK;
-  int rc;
-  if (p1) {
-    ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
-    ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
-    BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
-    ScopedTimer tm("decoder_bwd", stream);
-    if (use_tc) rc = decoder_bwd_tc_run(a, b, g, w, bw, stream);
-    else rc = (g.U == 4) ? launch_bwd<4>(a, g, bg, w, bw, d, stream) : launch_bwd<8>(a, g, bg, w, bw, d, stream);
-    if (rc) return rc;
-  }
-  ScopedTimer tmw("decoder_wgrad", stream);
-  if (p1) {
-    cond_kmajor_kernel<<<592, 256, 0, stream>>>(a, g, bw.COND);
-    count_launch();
-    ZCHECK_LAUNCH();
-  }
-  const long long sH = (long long)nbt * H * 32, s3 = (long long)nbt * 3 * H * 32, sX = (long long)nbt * K1P * 32, sC = (long long)nbt * C * 32;
-  const int nT = T - 1;
-  const int Kin = P_IN + a.Z;
-  // ---- CellStateEncoder backward (modules.py:238-243).  Its small GEMMs stage operands at the base of the scratch buffer, so on the
-  // folded path it runs BEFORE the bf16 history copies are laid out there (cse_tail = false afterwards)
-  auto cse_backward = [&]() -> int {
-    int r;
-    cse_gather_kernel<<<ceil_div(a.B * 2 * H, 256), 256, 0, stream>>>(a.B, H, bw.DH0, bw.DH1, bw.cse_dout);
-    count_launch();
-    r = sgemm_launch(1, 2 * H, H, a.B, bw.cse_dout, 2 * H, w.cse_h2, H, nullptr, b.dWc2, H, 0, 0, stream); if (r) return r;
-    colsum_kernel<<<ceil_div(2 * H, 256), 256, 0, stream>>>(bw.cse_dout, a.B, 2 * H, b.dbc2); count_launch();
-    r = gemm_f32_auto(2, a.B, H, 2 * H, bw.cse_dout, 2 * H, a.Wc2, H, nullptr, bw.cse_d2, H, 0, 0, stream); if (r) return r;
-    elu_bwd_kernel<<<ceil_div(a.B * H, 256), 256, 0, stream>>>(bw.cse_d2, w.cse_h2, (size_t)a.B * H); count_launch();
-    r = sgemm_launch(1, H, H, a.B, bw.cse_d2, H, w.cse_h1, H, nullptr, b.dWc1, H, 0, 0, stream); if (r) return r;
-    colsum_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d2, a.B, H, b.dbc1); count_launch();
-    r = gemm_f32_auto(2, a.B, H, H, bw.cse_d2, H, a.Wc1, H, nullptr, bw.cse_d1, H, 0, 0, stream); if (r) return r;
-    elu_bwd_kernel<<<ceil_div(a.B * H, 256), 256, 0, stream>>>(bw.cse_d1, w.cse_h1, (size_t)a.B * H); count_launch();
-    r = sgemm_launch(1, H, Kin, a.B, bw.cse_d1, H, w.cse_in, Kin, nullptr, b.dWc0, Kin, 0, 0, stream); if (r) return r;
-    colsum_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d1, a.B, H, b.dbc0); count_launch();
-    r = gemm_f32_auto(2, a.B, Kin, H, bw.cse_d1, H, a.Wc0, Kin, nullptr, bw.cse_din, Kin, 0, 0, stream); if (r) return r;
-    ZCHECK_LAUNCH();
-    return ZEGGS_OK;
-  };
-  bool cse_tail = true;
-  if (fold && p1) { if ((rc = cse_backward())) return rc; }
-  if (fold) cse_tail = false;
-  // ---- weight gradients (slots t = 1..T-1).  tensor-core path: every history is re-laid out once as bf16 (hi, lo)
-  // [rows][(T*nbt)*32] (contraction index contiguous) in the scratch buffer, then each dW is one NT GEMM with
-  // K = (T-1)*nbt*32; "previous step" operands are the same buffer shifted by one slot (32*nbt columns).
-  bool tc_done = false, dcond_rows = false;
-  if (gemm_mode() != 0 && scratch_base() != nullptr) {
-    // the tc engine's recurrence already runs on bf16 operands: a single bf16 pass matches its accuracy
-    const bool want_lo = gemm_mode() == 1 && !use_tc;
-    const int S = T * nbt;                       // slots per history
-    const size_t ld = (size_t)S * 32;
-    char* p = scratch_base();
-    struct Hist { const float* src; long long stride; int rows; __nv_bfloat16 *hi, *lo; float* db; };
-    Hist hs[11] = {
-      {bw.DY, sX, P_OUT, nullptr, nullptr, b.db2}, {bw.DGI1, s3, 3 * H, nullptr, nullptr, b.db_ih1}, {bw.DGH1, s3, 3 * H, nullptr, nullptr, b.db_hh1},
-      {bw.DGI0, s3, 3 * H, nullptr, nullptr, b.db_ih0}, {bw.DGH0, s3, 3 * H, nullptr, nullptr, b.db_hh0}, {bw.DPA, sH, H, nullptr, nullptr, b.db0},
-      {w.H0, sH, H, nullptr, nullptr, nullptr}, {w.H1, sH, H, nullptr, nullptr, nullptr}, {w.A, sH, H, nullptr, nullptr, nullptr},
-      {w.XP, sX, P_IN, nullptr, nullptr, nullptr}, {bw.COND, sC, C, nullptr, nullptr, nullptr}};
-    size_t need = 0;
-    for (auto& h : hs) need += (size_t)h.rows * ld * 2 * (want_lo ? 2 : 1);
-    // tc engine: the dpre_a / dgi0 histories are also needed transposed ([(t,b)][row], bf16) -- for the hoisted cond terms and
-    // for the x_pose gradient of the folded recurrence -- plus the transposed weight blocks and the DXP result
-    const size_t extra = fold ? (ld * H * 2 + ld * 3 * H * 2 + (size_t)C * 4 * H * 2 + (size_t)P_OUT * 4 * H * 2 + ld * P_OUT * 4 + 4096) : 0;
-    if (need + extra <= scratch_bytes()) {
-      // all hi parts first, then all lo parts: (ld * 2) bytes per row, 16 B aligned, so consecutive histories stack into ONE
-      // row-contiguous operand ([a | x_pose | cond] is the input of layer0 / GRU0 in the weights' own column order)
-      for (auto& h : hs) { h.hi = (__nv_bfloat16*)p; p += (size_t)h.rows * ld * 2; }
-      if (want_lo) for (auto& h : hs) { h.lo = (__nv_bfloat16*)p; p += (size_t)h.rows * ld * 2; }
-      auto takeq = [&](size_t bytes) { char* r = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255); p = r + bytes; return r; };
-      __nv_bfloat16 *paT = nullptr, *giT = nullptr, *w0T = nullptr, *wiT = nullptr, *w0xT = nullptr, *wixT = nullptr;
-      float* dxp = nullptr;
-      if (fold) {
-        paT = (__nv_bfloat16*)takeq(ld * H * 2); giT = (__nv_bfloat16*)takeq(ld * 3 * H * 2);
-        w0T = (__nv_bfloat16*)takeq((size_t)C * H * 2); wiT = (__nv_bfloat16*)takeq((size_t)C * 3 * H * 2);
-        w0xT = (__nv_bfloat16*)takeq((size_t)P_OUT * H * 2); wixT = (__nv_bfloat16*)takeq((size_t)P_OUT * 3 * H * 2);
-        dxp = (float*)takeq(ld * P_OUT * 4);
-      }
-      const int cur = nbt * 32;                  // column offset of slot t = 1
-      const int Kc = nT * nbt * 32;
-      // per-slot stride of the fp32 history is (stride / nbt) floats: slots (t,bt) are contiguous
-      // gradient histories: the same pass returns the bias gradient (sum over slots t >= 1, i.e. s >= nbt)
-      auto split = [&](Hist& h) { return split_hist_launch(h.src, h.stride / nbt, S, h.rows, h.hi, h.lo, stream, h.db, nbt); };
-      if (fold) {
-        if (p1) {
-          // ---- phase 1: d cond on the tensor cores (single-pass bf16): contract the transposed dpa / dgi0 histories with the transposed
-          // cond columns of W0 / W_ih0:  DCOND[(t,b)][c] = dpa^T W0[:, 1134+c] + dgi0^T W_ih0[:, H+1134+c]
-          if ((rc = split(hs[3]))) return rc;
-          if ((rc = split(hs[5]))) return rc;
-          if ((rc = transpose_bf16_launch(hs[5].hi, H, (int)ld, ld, paT, H, stream))) return rc;
-          if ((rc = transpose_bf16_launch(hs[3].hi, 3 * H, (int)ld, ld, giT, 3 * H, stream))) return rc;
-          if ((rc = split_t_launch(a.W0 + P_IN, H, C, A, w0T, nullptr, H, stream))) return rc;
-          if ((rc = split_t_launch(a.W_ih0 + H + P_IN, 3 * H, C, A + H, wiT, nullptr, 3 * H, stream))) return rc;
-          float* out = bw.DCOND + (size_t)cur * C;
-          if ((rc = tc_gemm_launch(Kc, C, H, paT + (size_t)cur * H, nullptr, H, w0T, nullptr, H, nullptr, out, C, 0, 0, stream))) return rc;
-          if ((rc = tc_gemm_launch(Kc, C, 3 * H, giT + (size_t)cur * 3 * H, nullptr, 3 * H, wiT, nullptr, 3 * H, nullptr, out, C, 0, 1, stream))) return rc;
-          dcond_scatter_kernel<<<592, 256, 0, stream>>>(a, g, bw.DCOND, bw.cse_din, b.dSpeech, b.dStyle, 1);
-          count_launch();
-          ZCHECK_LAUNCH();
-        }
-        dcond_rows = true;
-        if (p2) {
-          for (int hi_ : {1, 2, 4, 6, 7, 8, 9, 10}) if ((rc = split(hs[hi_]))) return rc;
-          // the x_pose gradient of every step at once (transposed dpre_a / dgi0 histories from phase 1):
-          //   DXP[(t,b)][n] = dpre_a(t)^T W0[:, n] + dgi0(t)^T W_ih0[:, H + n]      (n < 1131; modules.py:172-175 adjoint)
-          // and the layer-2 / x_pose gradient history the weight gradients read (modules.py:713, :728 adjoints):
-          //   DY[t][n][b] = out_std[n] (dY_ext[b][t][n] + DXP[(t+1,b)][n] / in_std[n] + [n < 6] dch(t)[b][n])
-          if ((rc = split_t_launch(a.W0, H, P_OUT, A, w0xT, nullptr, H, stream))) return rc;
-          if ((rc = split_t_launch(a.W_ih0 + H, 3 * H, P_OUT, A + H, wixT, nullptr, 3 * H, stream))) return rc;
-          if ((rc = tc_gemm_launch(Kc, P_OUT, H, paT + (size_t)cur * H, nullptr, H, w0xT, nullptr, H, nullptr, dxp + (size_t)cur * P_OUT, P_OUT, 0, 0, stream))) return rc;
-          if ((rc = tc_gemm_launch(Kc, P_OUT, 3 * H, giT + (size_t)cur * 3 * H, nullptr, 3 * H, wixT, nullptr, 3 * H, nullptr, dxp + (size_t)cur * P_OUT, P_OUT, 0, 1, stream))) return rc;
-          dy_combine_kernel<<<dim3(T - 1, ceil_div(P_OUT, 64)), 256, 0, stream>>>(a, b.dY, dxp, bw.DCH, bw.DY);
-          count_launch();
-          ZCHECK_LAUNCH();
-          if ((rc = split(hs[0]))) return rc;
-        }
-      } else {
-        for (auto& h : hs) if ((rc = split(h))) return rc;
-      }
-      if (p2) {
-        char* ws_p = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255);             // split-K partials behind the histories
-        const size_t ws_bytes = (size_t)(scratch_base() + scratch_bytes() - ws_p);
-        auto G = [&](const Hist& ga, int ga_off, int N, const Hist& xb, int xb_off, int K, float* dW, int ldw) {
-          return tc_gemm_launch(N, K, Kc, ga.hi + ga_off, want_lo ? ga.lo + ga_off : nullptr, (int)ld,
-                                xb.hi + xb_off, want_lo ? xb.lo + xb_off : nullptr, (int)ld, nullptr, dW, ldw, 0, 0, stream,
-                                (float*)ws_p, ws_bytes);
-        };
-        const Hist &hDY = hs[0], &hGI1 = hs[1], &hGH1 = hs[2], &hGI0 = hs[3], &hGH0 = hs[4], &hPA = hs[5], &hH0 = hs[6], &hH1 = hs[7],
-                   &hA = hs[8], &hXP = hs[9];
-        if ((rc = G(hDY, cur, P_OUT, hH1, cur, H, b.dW2, H))) return rc;
-        if ((rc = G(hGI1, cur, 3 * H, hH0, cur, H, b.dW_ih1, H))) return rc;
-        if ((rc = G(hGH1, cur, 3 * H, hH1, 0, H, b.dW_hh1, H))) return rc;
-        if ((rc = G(hGI0, cur, 3 * H, hA, cur, H + P_IN + C, b.dW_ih0, A + H))) return rc;     // [a | x_pose | cond] stacked
-        if ((rc = G(hGH0, cur, 3 * H, hH0, 0, H, b.dW_hh0, H))) return rc;
-        if ((rc = G(hPA, cur, H, hXP, cur, P_IN + C, b.dW0, A))) return rc;                    // [x_pose | cond] stacked
-      }
-      tc_done = true;
-    } else {
-      ZCHECK_ARG(!use_tc, "decoder bwd tc: scratch buffer too small for the batched gradient GEMMs (%zu bytes needed)", need + extra);
-    }
-  } else {
-    ZCHECK_ARG(!use_tc, "decoder bwd tc: needs the tensor-core GEMM front end (a zeggs_ctx with scratch, gemm mode 1 or 2)");
-  }
-  if (fold) return ZEGGS_OK;                    // the folded path is complete (CellStateEncoder + scatter ran in phase 1)
-#define WG(...) do { if (!tc_done) { rc = wgrad(__VA_ARGS__); if (rc) return rc; } } while (0)
-#define RS(...) do { if (!tc_done) { rc = rowsum(__VA_ARGS__); if (rc) return rc; } } while (0)
-  // layer2: dW2 = DY . H1[t]^T
-  WG(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, w.H1 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW2, H, stream);
-  RS(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, nT, nbt, b.db2, stream);
-  // GRU layer 1
-  WG(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih1, H, stream);
-  WG(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H1, sH, (long long)H * 32, H, nT, nbt, b.dW_hh1, H, stream);
-  RS(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih1, stream);
-  RS(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh1, stream);
-  // GRU layer 0: input = [a | x_pose | cond]
-  WG(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.A + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih0, A + H, stream);
-  WG(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW_ih0 + H, A + H, stream);
-  WG(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW_ih0 + H + P_IN, A + H, stream);
-  WG(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0, sH, (long long)H * 32, H, nT, nbt, b.dW_hh0, H, stream);
-  RS(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih0, stream);
-  RS(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh0, stream);
-  // layer0
-  WG(bw.DPA + sH, sH, (long long)H * 32, H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW0, A, stream);
-  WG(bw.DPA + sH, sH, (long long)H * 32, H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW0 + P_IN, A, stream);
-  RS(bw.DPA + sH, sH, (long long)H * 32, H, nT, nbt, b.db0, stream);
-#undef WG
-#undef RS
-  // ---- d cond[t] = W0[:, 1134:]^T dpre_a + W_ih0[:, H+1134:]^T dgi0   (batched over slots t >= 1)
-  if (!dcond_rows) {
-    rc = sgemm_batched_launch(1, C, 32, H, a.W0 + P_IN, A, bw.DPA + sH, 32, nullptr, bw.DCOND + sC, 32, 0, 0, nT * nbt, 0, (long long)H * 32, (long long)C * 32, stream); if (rc) return rc;
-    rc = sgemm_batched_launch(1, C, 32, 3 * H, a.W_ih0 + H + P_IN, A + H, bw.DGI0 + s3, 32, nullptr, bw.DCOND + sC, 32, 0, 1, nT * nbt, 0, (long long)3 * H * 32, (long long)C * 32, stream); if (rc) return rc;
-  }
-  if (cse_tail) { if ((rc = cse_backward())) return rc; }
-  dcond_scatter_kernel<<<592, 256, 0, stream>>>(a, g, bw.DCOND, bw.cse_din, b.dSpeech, b.dStyle, dcond_rows ? 1 : 0);
-  count_launch();
-  ZCHECK_LAUNCH();
-  return ZEGGS_OK;
+  // a tensor-core forward with no BPTT pack (packed_bwd_tc == NULL) takes the fp32 backward
+  if (a.engine == 1 && b.packed_bwd_tc) return decoder_window_bwd_tc(a, b, g, w, bw, stream);
+  return decoder_window_bwd_fp32(a, b, g, w, bw, stream);
 }
 
 }  // namespace zeggs

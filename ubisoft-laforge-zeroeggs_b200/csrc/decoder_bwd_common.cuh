@@ -78,8 +78,34 @@ __device__ __forceinline__ void gru_gate_bwd(float dh, float r, float z, float n
   dgh[0] = dpr; dgh[1] = dpz; dgh[2] = dpn * r;
 }
 
-
-int decoder_bwd_tc_run(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
-                       const BwdWs& bw, cudaStream_t stream);
+// ------------------------------------------------------------------ host steps shared by the two backward routines
+// Weight gradients (slots t = 1..T-1) on the tensor cores: each of the 11 fp32 histories is re-laid out once as bf16 hi (and lo)
+// [rows][T*nbt*32] (contraction index contiguous) from the base of the scratch buffer, all hi parts first, then all lo parts.  (ld * 2)
+// bytes per row keep every copy 16 B aligned, so consecutive histories stack into ONE row-contiguous operand ([a | x_pose | cond] is
+// the input of layer0 / GRU0 in the weights' own column order).  Each dW is one NT GEMM with K = (T-1)*nbt*32; "previous step"
+// operands are the same copy shifted by one slot (32*nbt columns).
+enum { HDY, HGI1, HGH1, HGI0, HGH0, HPA, HH0, HH1, HA, HXP, HCOND, NHIST };
+struct WgradHist { const float* src; long long stride; int rows; __nv_bfloat16 *hi, *lo; float* db; };   // db: bias gradient
+struct WgradHists {
+  WgradHist h[NHIST];
+  int slots, nbt;     // slots per history (T * nbt), batch tiles
+  size_t ld, bytes;   // columns of every copy (slots * 32), bytes of all copies
+  char* end;          // first scratch byte behind them
+};
+// The table and the carve-up, host arithmetic only: calls with the same geometry and scratch buffer return the same addresses.
+WgradHists wgrad_hists(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
+                       const BwdWs& bw, bool want_lo);
+int split_hist(const WgradHists& hs, int i, cudaStream_t stream);
+// the six GEMMs; split-K partials go to the scratch bytes from `tail` on
+int wgrad_gemms(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const WgradHists& hs, bool want_lo,
+                char* tail, cudaStream_t stream);
+int cond_kmajor(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdWs& bw, cudaStream_t stream);
+// CellStateEncoder backward (modules.py:238-243); its small GEMMs stage operands at the base of the scratch buffer
+int cse_backward(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecWs& w, const BwdWs& bw, cudaStream_t stream);
+int dcond_scatter(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const BwdWs& bw, int rows,
+                  cudaStream_t stream);
+int dy_combine(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const float* dxp, const BwdWs& bw, cudaStream_t stream);
+int decoder_window_bwd_tc(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
+                          const BwdWs& bw, cudaStream_t stream);
 
 }  // namespace zeggs

@@ -28,7 +28,7 @@
 //   B4  A = d pre_a image [32 x H], B = [Mfold_a^T | Wgz_a^T]                  -> fold / gaze parts -> R(t-1): root adjoint,
 //                                                                                  dh1(t-1) -> GRU1 gate adjoint -> G1 image
 // The x_pose / layer-2 gradient history the weight gradients need (DY) is rebuilt after the recurrence by two batched
-// GEMMs over the transposed dpre_a / dgi0 histories (decoder_bwd.cu).
+// GEMMs over the transposed dpre_a / dgi0 histories (decoder_window_bwd_tc).
 // fp32 histories for the weight gradients are written in the same k-major layout as the SIMT kernel, so the batched
 // wgrad code is shared.
 #include "decoder_bwd_common.cuh"
@@ -584,33 +584,97 @@ static int launch_bt(const zeggs_decoder_fwd_args& a, const DecGeom& g, const Bw
   return ZEGGS_OK;
 }
 
-int decoder_bwd_tc_run(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
-                       const BwdWs& bw, cudaStream_t stream) {
-  BwdGeom bg = make_bgeom(g);
-  ZCHECK_ARG(g.nbt == 1, "decoder bwd tc engine needs B <= 32 (got B=%d)", a.B);
-  ZCHECK_ARG(b.packed_bwd_tc && b.workspace_tc, "decoder bwd tc: packed_bwd_tc / workspace_tc missing");
-  BtGeom tg = make_btgeom(g, bg);
-  ZCHECK_ARG((tg.kbH % 2) == 0, "decoder bwd tc: unsupported geometry");
-  BtWs iw = make_btws(b.workspace_tc, g);
-  iw.dbg = tc_debug_buffer();
-  iw.dch = bw.DCH;
-  // PRE[(b,t)][j] = sum_n W2[n][j] out_std[n] dY[b][t][n]: the layer-2 adjoint of the external gradient for every frame at once
-  const int H = a.H, ld = round_up(P_OUT, 8);
-  const size_t rows = (size_t)a.B * a.T;
+// Tensor-core engine backward.  Phase 0 runs all of it.  Phase 1 runs the BPTT recurrence, the CellStateEncoder backward and the
+// conditioning gradients (dSpeech, dStyle); phase 2 every remaining parameter gradient.  Split in two calls, the encoders' backward
+// passes (which need only dSpeech / dStyle) can overlap the large weight-gradient GEMMs on other streams.  Phase 2 reads the history
+// copies phase 1 left in the scratch buffer, which wgrad_hists and the carve-up below place at the same addresses in both calls.
+int decoder_window_bwd_tc(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
+                          const BwdWs& bw, cudaStream_t stream) {
+  const int H = a.H, T = a.T, C = a.S + a.Z, A = g.A, phase = b.phase;
+  const BwdGeom bg = make_bgeom(g);
+  const BtGeom tg = make_btgeom(g, bg);
+  ZCHECK_SUPPORTED(tc_hidden_ok(H), "decoder bwd tc: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", H);
+  ZCHECK_ARG(g.nbt == 1 && bg.n4b == 1, "decoder bwd tc engine needs B <= 32 (got B=%d)", a.B);
+  ZCHECK_ARG(b.workspace_tc, "decoder bwd tc: workspace_tc missing");
+  ZCHECK_ARG(gemm_mode() != 0 && scratch_base() != nullptr,
+             "decoder bwd tc: needs the tensor-core GEMM front end (a zeggs_ctx with scratch, gemm mode 1 or 2)");
+  // PRE[(b,t)][j] = sum_n W2[n][j] out_std[n] dY[b][t][n]: the layer-2 adjoint of the external gradient for every frame at once,
+  // operands and result at the scratch base for the duration of the recurrence
+  const int ldy = round_up(P_OUT, 8);
+  const size_t rows = (size_t)a.B * T;
   char* p = scratch_base();
-  ZCHECK_ARG(p != nullptr, "decoder bwd tc: scratch buffer missing (zeggs_ctx.scratch)");
   auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) / 256 * 256; return r; };
-  __nv_bfloat16* dys = (__nv_bfloat16*)take(rows * ld * 2);
-  __nv_bfloat16* w2t = (__nv_bfloat16*)take((size_t)H * ld * 2);
+  __nv_bfloat16* dys = (__nv_bfloat16*)take(rows * ldy * 2);
+  __nv_bfloat16* w2t = (__nv_bfloat16*)take((size_t)H * ldy * 2);
   float* pre = (float*)take(rows * H * sizeof(float));
   ZCHECK_ARG((size_t)(p - scratch_base()) <= scratch_bytes(), "decoder bwd tc: scratch buffer too small (%zu bytes needed)", (size_t)(p - scratch_base()));
-  dy_scale_bf16_kernel<<<1184, 256, 0, stream>>>(b.dY, a.out_std, rows, ld, dys); count_launch();
-  int rc = split_t_launch(a.W2, P_OUT, H, H, w2t, nullptr, ld, stream); if (rc) return rc;
-  rc = tc_gemm_launch((int)rows, H, ld, dys, nullptr, ld, w2t, nullptr, ld, nullptr, pre, H, 0, 0, stream); if (rc) return rc;
-  iw.pre = pre;
-  BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = nullptr;
-  return g.U == 4 ? launch_bt<4>(a, g, bg, tg, w, bw, iw, d, (const uint8_t*)b.packed_bwd_tc, stream)
-                  : launch_bt<8>(a, g, bg, tg, w, bw, iw, d, (const uint8_t*)b.packed_bwd_tc, stream);
+  // the weight gradients: single-pass bf16 history copies (the recurrence already runs on bf16 operands, so one pass matches its
+  // accuracy), and behind them the dpa / dgi0 copies transposed to [(t,b)][row] (A operands of the d cond and x_pose gradient GEMMs),
+  // the transposed cond / x_pose columns of W0 / W_ih0 and the DXP result
+  const WgradHists hs = wgrad_hists(a, b, g, w, bw, false);
+  const size_t ld = hs.ld;
+  const size_t extra = ld * H * 2 + ld * 3 * H * 2 + (size_t)C * 4 * H * 2 + (size_t)P_OUT * 4 * H * 2 + ld * P_OUT * 4 + 4096;
+  ZCHECK_ARG(hs.bytes + extra <= scratch_bytes(), "decoder bwd tc: scratch buffer too small for the batched gradient GEMMs (%zu bytes needed)",
+             hs.bytes + extra);
+  char* q = hs.end;
+  auto takeq = [&](size_t bytes) { char* r = (char*)(((uintptr_t)q + 255) & ~(uintptr_t)255); q = r + bytes; return r; };
+  __nv_bfloat16* paT = (__nv_bfloat16*)takeq(ld * H * 2);
+  __nv_bfloat16* giT = (__nv_bfloat16*)takeq(ld * 3 * H * 2);
+  __nv_bfloat16* w0T = (__nv_bfloat16*)takeq((size_t)C * H * 2);
+  __nv_bfloat16* wiT = (__nv_bfloat16*)takeq((size_t)C * 3 * H * 2);
+  __nv_bfloat16* w0xT = (__nv_bfloat16*)takeq((size_t)P_OUT * H * 2);
+  __nv_bfloat16* wixT = (__nv_bfloat16*)takeq((size_t)P_OUT * 3 * H * 2);
+  float* dxp = (float*)takeq(ld * P_OUT * 4);
+  const int cur = 32;                    // row of (t = 1, b = 0) in the transposed copies, column of slot t = 1 in the others
+  const int Kc = (T - 1) * 32;
+  int rc;
+  if (phase != 2) {
+    ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
+    ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * K1P * 32 * sizeof(float), stream));
+    ScopedTimer tm("decoder_bwd", stream);
+    dy_scale_bf16_kernel<<<1184, 256, 0, stream>>>(b.dY, a.out_std, rows, ldy, dys); count_launch();
+    if ((rc = split_t_launch(a.W2, P_OUT, H, H, w2t, nullptr, ldy, stream))) return rc;
+    if ((rc = tc_gemm_launch((int)rows, H, ldy, dys, nullptr, ldy, w2t, nullptr, ldy, nullptr, pre, H, 0, 0, stream))) return rc;
+    BtWs iw = make_btws(b.workspace_tc, g);
+    iw.dbg = tc_debug_buffer();
+    iw.dch = bw.DCH;
+    iw.pre = pre;
+    BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = nullptr;
+    const uint8_t* pk = (const uint8_t*)b.packed_bwd_tc;
+    rc = g.U == 4 ? launch_bt<4>(a, g, bg, tg, w, bw, iw, d, pk, stream) : launch_bt<8>(a, g, bg, tg, w, bw, iw, d, pk, stream);
+    if (rc) return rc;
+  }
+  ScopedTimer tm("decoder_wgrad", stream);
+  if (phase != 2) {
+    if ((rc = cond_kmajor(a, g, bw, stream))) return rc;
+    // before the history copies overwrite its staging area at the scratch base
+    if ((rc = cse_backward(a, b, w, bw, stream))) return rc;
+    // d cond on the tensor cores: DCOND[(t,b)][c] = dpa^T W0[:, 1134+c] + dgi0^T W_ih0[:, H+1134+c]
+    if ((rc = split_hist(hs, HGI0, stream))) return rc;
+    if ((rc = split_hist(hs, HPA, stream))) return rc;
+    if ((rc = transpose_bf16_launch(hs.h[HPA].hi, H, (int)ld, ld, paT, H, stream))) return rc;
+    if ((rc = transpose_bf16_launch(hs.h[HGI0].hi, 3 * H, (int)ld, ld, giT, 3 * H, stream))) return rc;
+    if ((rc = split_t_launch(a.W0 + P_IN, H, C, A, w0T, nullptr, H, stream))) return rc;
+    if ((rc = split_t_launch(a.W_ih0 + H + P_IN, 3 * H, C, A + H, wiT, nullptr, 3 * H, stream))) return rc;
+    float* out = bw.DCOND + (size_t)cur * C;
+    if ((rc = tc_gemm_launch(Kc, C, H, paT + (size_t)cur * H, nullptr, H, w0T, nullptr, H, nullptr, out, C, 0, 0, stream))) return rc;
+    if ((rc = tc_gemm_launch(Kc, C, 3 * H, giT + (size_t)cur * 3 * H, nullptr, 3 * H, wiT, nullptr, 3 * H, nullptr, out, C, 0, 1, stream))) return rc;
+    if ((rc = dcond_scatter(a, b, g, bw, 1, stream))) return rc;
+  }
+  if (phase != 1) {
+    for (int i : {HGI1, HGH1, HGH0, HH0, HH1, HA, HXP, HCOND}) if ((rc = split_hist(hs, i, stream))) return rc;
+    // the x_pose gradient of every step at once, from the transposed dpre_a / dgi0 copies of phase 1:
+    //   DXP[(t,b)][n] = dpre_a(t)^T W0[:, n] + dgi0(t)^T W_ih0[:, H + n]      (n < 1131; modules.py:172-175 adjoint)
+    // then the layer-2 / x_pose gradient history the weight gradients read (modules.py:713, :728 adjoints)
+    if ((rc = split_t_launch(a.W0, H, P_OUT, A, w0xT, nullptr, H, stream))) return rc;
+    if ((rc = split_t_launch(a.W_ih0 + H, 3 * H, P_OUT, A + H, wixT, nullptr, 3 * H, stream))) return rc;
+    if ((rc = tc_gemm_launch(Kc, P_OUT, H, paT + (size_t)cur * H, nullptr, H, w0xT, nullptr, H, nullptr, dxp + (size_t)cur * P_OUT, P_OUT, 0, 0, stream))) return rc;
+    if ((rc = tc_gemm_launch(Kc, P_OUT, 3 * H, giT + (size_t)cur * 3 * H, nullptr, 3 * H, wixT, nullptr, 3 * H, nullptr, dxp + (size_t)cur * P_OUT, P_OUT, 0, 1, stream))) return rc;
+    if ((rc = dy_combine(a, b, dxp, bw, stream))) return rc;
+    if ((rc = split_hist(hs, HDY, stream))) return rc;
+    if ((rc = wgrad_gemms(a, b, g, hs, false, q, stream))) return rc;
+  }
+  return ZEGGS_OK;
 }
 
 }  // namespace zeggs

@@ -146,7 +146,6 @@ inline DecWs make_ws(void* base, const DecGeom& g, int T, int save) {
 }
 
 const float* decoder_tc_mfold(const zeggs_decoder_fwd_args& a);   // fp32 [4H][H] fold matrix inside packed_tc
-int decoder_fwd_tc_hoist(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream);
 int decoder_fwd_tc_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream);
 
 // ------------------------------------------------------------------ skinny GEMM

@@ -139,19 +139,6 @@ __global__ void __launch_bounds__(256) cond_precompute_kernel(zeggs_decoder_fwd_
   }
 }
 
-// cond rows for the tc engine: R[(t*32 + b)][c] = [speech[b,t,:] | style[b,t,:]] (zero rows for b >= B)
-__global__ void cond_rows_kernel(zeggs_decoder_fwd_args a, float* __restrict__ R) {
-  const int C = a.S + a.Z, T = a.T;
-  const size_t total = (size_t)T * 32 * C;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int cc = (int)(i % C); const size_t e = i / C;
-    const int b = (int)(e & 31), t = (int)(e >> 5);
-    float v = 0.f;
-    if (b < a.B) v = cc < a.S ? a.speech[((size_t)b * T + t) * a.S + cc] : a.style[((size_t)b * T + t) * a.Z + (cc - a.S)];
-    R[i] = v;
-  }
-}
-
 // ------------------------------------------------------------------ the persistent kernel
 template <int U>
 __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, DecWs w) {
@@ -355,6 +342,18 @@ static int launch_fwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const D
   return ZEGGS_OK;
 }
 
+// fp32 engine: the hoisted speech / style terms, then the SIMT recurrence
+static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
+  const int C = a.S + a.Z;
+  const size_t sm = (size_t)(C * 33 + 64 * (C + 1)) * sizeof(float);
+  ZCHECK_CUDA(cudaFuncSetAttribute(cond_precompute_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  cond_precompute_kernel<<<dim3(a.T, g.nbt, ceil_div(4 * a.H, 64)), 256, sm, stream>>>(a, g, w.S01);
+  count_launch();
+  ZCHECK_LAUNCH();
+  ScopedTimer tm("decoder_fwd", stream);
+  return g.U == 4 ? launch_fwd<4>(a, g, w, stream) : launch_fwd<8>(a, g, w, stream);
+}
+
 extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* stream_) {
   int rc = check_fwd_args(ap); if (rc) return rc;
   const zeggs_decoder_fwd_args& a = *ap;
@@ -370,8 +369,7 @@ extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* 
   ZCHECK_CUDA(cudaMemsetAsync(w.XP, 0, (size_t)w.TS * g.nbt * K1P * 32 * sizeof(float), stream));
   ZCHECK_CUDA(cudaMemsetAsync(w.H0, 0, (size_t)g.nbt * a.H * 32 * sizeof(float), stream));
   ZCHECK_CUDA(cudaMemsetAsync(w.H1, 0, (size_t)g.nbt * a.H * 32 * sizeof(float), stream));
-  const int slot1 = w.save ? 1 : 1;
-  decoder_prologue_kernel<<<a.B, 256, 0, stream>>>(a, g, w.cse_in, w.XP + (size_t)slot1 * g.nbt * K1P * 32);
+  decoder_prologue_kernel<<<a.B, 256, 0, stream>>>(a, g, w.cse_in, w.XP + (size_t)g.nbt * K1P * 32);
   count_launch();
   ZCHECK_LAUNCH();
   // CellStateEncoder (modules.py:238-243)
@@ -381,29 +379,8 @@ extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* 
   cse_scatter_kernel<<<ceil_div(a.B * 2 * a.H, 256), 256, 0, stream>>>(a.B, a.H, w.cse_out, w.H0, w.H1);
   count_launch();
   ZCHECK_LAUNCH();
-  if (a.T > 1) {
-    const int C = a.S + a.Z;
-    size_t sm = (size_t)(C * 33 + 64 * (C + 1)) * sizeof(float);
-    if (a.engine == 1) {
-      // hoisted speech/style terms as two GEMMs (tensor cores when a scratch buffer is set): S01[(t,b)][4H] =
-      // cond_rows [(t,b)][C] . [W0[:, 1134:] ; W_ih0[:, H+1134:]]^T + [b0 ; b_ih0]
-      ZCHECK_ARG(g.nbt == 1, "decoder tc engine handles one 32-sample batch tile (B <= 32); got B=%d", a.B);
-      cond_rows_kernel<<<592, 256, 0, stream>>>(a, w.CONDR);
-      count_launch();
-      ZCHECK_LAUNCH();
-      rc = decoder_fwd_tc_hoist(a, g, w, stream); if (rc) return rc;
-      rc = decoder_fwd_tc_run(a, g, w, stream);
-    } else {
-      ZCHECK_CUDA(cudaFuncSetAttribute(cond_precompute_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      cond_precompute_kernel<<<dim3(a.T, g.nbt, ceil_div(4 * a.H, 64)), 256, sm, stream>>>(a, g, w.S01);
-      count_launch();
-      ZCHECK_LAUNCH();
-      ScopedTimer tm("decoder_fwd", stream);
-      if (g.U == 4) rc = launch_fwd<4>(a, g, w, stream); else rc = launch_fwd<8>(a, g, w, stream);
-    }
-    if (rc) return rc;
-  }
-  return ZEGGS_OK;
+  if (a.T == 1) return ZEGGS_OK;
+  return a.engine == 1 ? decoder_fwd_tc_run(a, g, w, stream) : decoder_fwd_fp32_run(a, g, w, stream);
 }
 
 }  // namespace zeggs

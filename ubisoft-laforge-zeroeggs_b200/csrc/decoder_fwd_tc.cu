@@ -626,6 +626,19 @@ __global__ void __launch_bounds__(256) fold_finish_kernel(zeggs_decoder_fwd_args
   }
 }
 
+// cond rows for the tc engine: R[(t*32 + b)][c] = [speech[b,t,:] | style[b,t,:]] (zero rows for b >= B)
+__global__ void cond_rows_kernel(zeggs_decoder_fwd_args a, float* __restrict__ R) {
+  const int C = a.S + a.Z, T = a.T;
+  const size_t total = (size_t)T * 32 * C;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int cc = (int)(i % C); const size_t e = i / C;
+    const int b = (int)(e & 31), t = (int)(e >> 5);
+    float v = 0.f;
+    if (b < a.B) v = cc < a.S ? a.speech[((size_t)b * T + t) * a.S + cc] : a.style[((size_t)b * T + t) * a.Z + (cc - a.S)];
+    R[i] = v;
+  }
+}
+
 // ------------------------------------------------------------------ host
 extern "C" size_t zeggs_decoder_packed_tc_bytes(int H, int S, int Z) {
   if (!tc_hidden_ok(H)) return 0;
@@ -704,29 +717,26 @@ static long long* g_tc_dbg = nullptr;
 long long* tc_debug_buffer() { return g_tc_dbg; }
 extern "C" void zeggs_debug_set_tc_trace(void* p) { g_tc_dbg = (long long*)p; }
 
-// hoisted terms of the tc engine: S01[(t,b)][4H] = cond rows . [W0[:, 1134:] ; W_ih0[:, H+1134:]]^T + bfold, then the first
-// step's pose contribution (called by zeggs_decoder_window_fwd after the prologue / CellStateEncoder)
-int decoder_fwd_tc_hoist(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
+// tc engine after the prologue / CellStateEncoder of zeggs_decoder_window_fwd, which has checked tc_hidden_ok(H): the hoisted speech /
+// style terms, the recurrence, then layer 2 of every step at once
+int decoder_fwd_tc_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
   TcGeom tg = make_tcgeom(g);
-  ZCHECK_ARG(a.packed_tc, "decoder tc: packed_tc missing");
-  const uint8_t* base = (const uint8_t*)a.packed_tc;
-  const float* cfold = (const float*)(base + tg.off_cfold);
-  const float* bfold = (const float*)(base + tg.off_bfold);
+  ZCHECK_ARG(g.nbt == 1, "decoder tc engine handles one 32-sample batch tile (B <= 32); got B=%d", a.B);
+  ZCHECK_ARG(a.packed_tc && a.workspace_tc, "decoder tc: packed_tc / workspace_tc missing");
+  const uint8_t* pk = (const uint8_t*)a.packed_tc;
+  const float* cfold = (const float*)(pk + tg.off_cfold);
+  const float* bfold = (const float*)(pk + tg.off_bfold);
   const int C = a.S + a.Z, H = a.H;
+  // hoisted terms: S01[(t,b)][4H] = cond rows [(t,b)][C] . [W0[:, 1134:] ; W_ih0[:, H+1134:]]^T + bfold, then the first step's pose
+  // contribution
+  cond_rows_kernel<<<592, 256, 0, stream>>>(a, w.CONDR);
+  count_launch();
+  ZCHECK_LAUNCH();
   int rc = gemm_f32_auto(0, a.T * 32, H, C, w.CONDR, C, a.W0 + P_IN, g.A, bfold, w.S01, 4 * H, 0, 0, stream); if (rc) return rc;
   rc = gemm_f32_auto(0, a.T * 32, 3 * H, C, w.CONDR, C, a.W_ih0 + H + P_IN, g.A + H, bfold + H, w.S01 + H, 4 * H, 0, 0, stream); if (rc) return rc;
   fold_first_step_kernel<<<ceil_div(4 * H, 8), 256, 0, stream>>>(H, g.A, a.W0, a.W_ih0, w.XP + (size_t)K1P * 32, cfold, w.S01 + (size_t)32 * 4 * H);
   count_launch();
   ZCHECK_LAUNCH();
-  return ZEGGS_OK;
-}
-
-// called by zeggs_decoder_window_fwd after the prologue / CellStateEncoder / hoisted terms when engine == 1
-int decoder_fwd_tc_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
-  TcGeom tg = make_tcgeom(g);
-  ZCHECK_ARG(g.nbt == 1, "decoder tc engine handles one 32-sample batch tile (B <= 32); got B=%d", a.B);
-  ZCHECK_ARG(a.packed_tc && a.workspace_tc, "decoder tc: packed_tc / workspace_tc missing");
-  ZCHECK_ARG(a.H % 64 == 0 && tg.kbH <= 16, "decoder tc: unsupported hidden size %d", a.H);
   TcWs tw = make_tcws(a.workspace_tc, g);
   tw.dbg = g_tc_dbg;
   // images of h0(0), h1(0) from the fp32 k-major buffers the CellStateEncoder wrote
@@ -734,13 +744,11 @@ int decoder_fwd_tc_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const 
   image_from_kmajor_kernel<<<64, 256, 0, stream>>>(w.H1, a.H, tg.kbH, tw.h1b[0]); count_launch();
   ZCHECK_LAUNCH();
   ScopedTimer tm("decoder_fwd", stream);
-  int rc;
-  const uint8_t* pk = (const uint8_t*)a.packed_tc;
   rc = g.U == 4 ? launch_tc<4>(a, g, tg, w, tw, pk, stream) : launch_tc<8>(a, g, tg, w, tw, pk, stream);
   if (rc) return rc;
   // layer2 for every step at once: YC[(t,b)][:] = h1(t) W2^T + b2 over the bf16 history (rows t = 1..T-1)
   const __nv_bfloat16* h1b = reinterpret_cast<const __nv_bfloat16*>(w.H1B) + (size_t)32 * a.H;
-  const __nv_bfloat16* w2b = reinterpret_cast<const __nv_bfloat16*>((const uint8_t*)a.packed_tc + tg.off_w2b);
+  const __nv_bfloat16* w2b = reinterpret_cast<const __nv_bfloat16*>(pk + tg.off_w2b);
   rc = tc_gemm_launch((a.T - 1) * 32, P_OUT, a.H, h1b, nullptr, a.H, w2b, nullptr, a.H, a.b2, w.YC, P_OUT, 0, 0, stream); if (rc) return rc;
   const int nch = ceil_div(P_OUT, 64);
   fold_finish_kernel<<<dim3(a.T - 1, nch), 256, 0, stream>>>(a, w, nch);

@@ -179,6 +179,24 @@ def split_pose(Y, root_pos, root_rot):
             Y[..., o + NJ * 12:o + NJ * 15].reshape(B, T, NJ, 3))
 
 
+def _weight_pack(dec, kind, a, dev):
+    """Device buffer of the decoder's weight pack `kind` -- "" (fp32 forward), "_tc", "_bwd" or "_bwd_tc": the output of
+    zeggs_decoder_pack_weights<kind> -- cached on the module as `_zeggs_packed<kind>` and re-packed whenever any parameter's version
+    counter moved or the device changed."""
+    l = _lib.lib()
+    ver = weights_key(dec._weights())
+    cache = dec.__dict__.get("_zeggs_packed" + kind)
+    if cache is None or cache[0] != ver or cache[1].device != dev:
+        nbytes = getattr(l, f"zeggs_decoder_packed{kind}_bytes")(a.H, a.S, a.Z)
+        if nbytes == 0:
+            raise _lib.ZeggsError(f"decoder hidden size {a.H} unsupported")
+        packed = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        name = f"zeggs_decoder_pack_weights{kind}"
+        _lib.check(getattr(l, name)(a, packed.data_ptr(), _lib.stream_ptr()), name)
+        cache = dec.__dict__["_zeggs_packed" + kind] = (ver, packed)
+    return cache[1]
+
+
 def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
     """Fill a DecoderFwdArgs; returns (args, keepalive list).  pack_only: stop after the weight packs (decoder_prepack)."""
     H, S, Z = dec.hidden_size, dec.speech_encoding_size, dec.style_encoding_size
@@ -197,34 +215,19 @@ def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
     for n, t in tensors.items():
         setattr(a, n, _lib.ptr(t))
         keep.append(t)
-    # packed weights: re-packed whenever any parameter's version counter moved (each engine packs only its own slices)
-    ver = weights_key(dec._weights())
+    # each engine packs only its own slices
     use_tc = resolve_engine(H, S, Z)
     if use_tc and B > 32:
         raise _lib.ZeggsError("tensor-core decoder engine: one call covers one 32-sample batch tile (decoder_window splits larger batches)")
-    if not use_tc:
-        cache = getattr(dec, "_zeggs_packed", None)
-        if cache is None or cache[0] != ver or cache[1].device != dev:
-            nbytes = l.zeggs_decoder_packed_bytes(H, S, Z)
-            if nbytes == 0:
-                raise _lib.ZeggsError(f"decoder hidden size {H} unsupported")
-            packed = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
-            _lib.check(l.zeggs_decoder_pack_weights(a, packed.data_ptr(), _lib.stream_ptr()), "zeggs_decoder_pack_weights")
-            dec.__dict__["_zeggs_packed"] = (ver, packed)
-            cache = dec.__dict__["_zeggs_packed"]
-        a.packed = cache[1].data_ptr()
-        keep.append(cache[1])
     if use_tc:
-        tcc = dec.__dict__.get("_zeggs_packed_tc")
-        if tcc is None or tcc[0] != ver or tcc[1].device != dev:
-            nb = l.zeggs_decoder_packed_tc_bytes(H, S, Z)
-            ptc = torch.empty(nb, dtype=torch.uint8, device=dev)
-            _lib.check(l.zeggs_decoder_pack_weights_tc(a, ptc.data_ptr(), _lib.stream_ptr()), "zeggs_decoder_pack_weights_tc")
-            dec.__dict__["_zeggs_packed_tc"] = (ver, ptc)
-            tcc = dec.__dict__["_zeggs_packed_tc"]
+        ptc = _weight_pack(dec, "_tc", a, dev)
         wtc = WS.get("dec_tc", l.zeggs_decoder_tc_workspace_bytes(H, S, Z), dev)
-        a.engine, a.packed_tc, a.workspace_tc = 1, tcc[1].data_ptr(), wtc.data_ptr()
-        keep += [tcc[1], wtc]
+        a.engine, a.packed_tc, a.workspace_tc = 1, ptc.data_ptr(), wtc.data_ptr()
+        keep += [ptc, wtc]
+    else:
+        packed = _weight_pack(dec, "", a, dev)
+        a.packed = packed.data_ptr()
+        keep.append(packed)
     if pack_only:
         return a, keep, None
     wsb = l.zeggs_decoder_workspace_bytes(B, T, H, S, Z, int(save))
@@ -240,24 +243,10 @@ def decoder_prepack(dec, B, T, dev, stats, dt, backward=True):
     """Everything the decoder derives from its WEIGHTS alone -- the engine's packed / bf16 weight images, the folded layer-2 matrix and
     (backward=True) the transposed images of the BPTT kernel -- issued on the current stream and lane.  The window calls find the caches
     fresh and skip the work, so a training step can run this next to the encoders' forward instead of in front of the recurrence."""
-    l = _lib.lib()
     a, keep, _ = _decoder_args(dec, B, T, dev, {}, stats, dt, False, pack_only=True)
     if backward and a.engine == 1:
-        _pack_bwd_tc(dec, a, dev)
+        _weight_pack(dec, "_bwd_tc", a, dev)
     return keep
-
-
-def _pack_bwd_tc(dec, a, dev):
-    l = _lib.lib()
-    H, S, Z = a.H, a.S, a.Z
-    ver = weights_key(dec._weights())
-    tcc = dec.__dict__.get("_zeggs_packed_bwd_tc")
-    if tcc is None or tcc[0] != ver or tcc[1].device != dev:
-        ptc = torch.empty(l.zeggs_decoder_packed_bwd_tc_bytes(H, S, Z), dtype=torch.uint8, device=dev)
-        _lib.check(l.zeggs_decoder_pack_weights_bwd_tc(a, ptc.data_ptr(), _lib.stream_ptr()), "zeggs_decoder_pack_weights_bwd_tc")
-        dec.__dict__["_zeggs_packed_bwd_tc"] = (ver, ptc)
-        tcc = dec.__dict__["_zeggs_packed_bwd_tc"]
-    return tcc
 
 
 def decoder_window_forward(dec, root_pos0, root_rot0, pose0, gaze_pos, speech, style, stats, dt, save=False):
@@ -312,26 +301,16 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
             g = g.contiguous().float()
             hold.append(g)
             setattr(b, name, g.data_ptr())
-    # transposed weight slices for the backward recurrence (cached on the module like the forward pack)
-    ver = weights_key(dec._weights())
-    use_tc = a.engine == 1
-    if use_tc and l.zeggs_decoder_packed_bwd_tc_bytes(H, S, Z) == 0:
-        raise _lib.ZeggsError(f"tensor-core decoder backward unavailable for hidden size {H}")
-    if not use_tc:
-        cache = dec.__dict__.get("_zeggs_packed_bwd")
-        if cache is None or cache[0] != ver or cache[1].device != dev:
-            nb = l.zeggs_decoder_packed_bwd_bytes(H, S, Z)
-            packed = torch.empty(nb // 4, dtype=torch.float32, device=dev)
-            _lib.check(l.zeggs_decoder_pack_weights_bwd(a, packed.data_ptr(), _lib.stream_ptr()), "zeggs_decoder_pack_weights_bwd")
-            dec.__dict__["_zeggs_packed_bwd"] = (ver, packed)
-            cache = dec.__dict__["_zeggs_packed_bwd"]
-        b.packed_bwd = cache[1].data_ptr()
-        hold.append(cache[1])
-    else:
-        tcc = _pack_bwd_tc(dec, a, dev)
+    # transposed weight slices for the backward recurrence
+    if a.engine == 1:
+        ptc = _weight_pack(dec, "_bwd_tc", a, dev)
         wtc = WS.get("dec_bwd_tc", l.zeggs_decoder_bwd_tc_workspace_bytes(H, S, Z), dev)
-        b.packed_bwd_tc, b.workspace_tc = tcc[1].data_ptr(), wtc.data_ptr()
-        hold += [tcc[1], wtc]
+        b.packed_bwd_tc, b.workspace_tc = ptc.data_ptr(), wtc.data_ptr()
+        hold += [ptc, wtc]
+    else:
+        packed = _weight_pack(dec, "_bwd", a, dev)
+        b.packed_bwd = packed.data_ptr()
+        hold.append(packed)
     grads = _grad_targets(dec._weights(), grads_out)
     for n, g in zip(_DEC_GRAD_NAMES, grads):
         setattr(b, n, g.data_ptr())
