@@ -55,7 +55,7 @@ int zeggs_timing_read(const char* name, double* total_ms, int* count);
 typedef struct {
   void* scratch;          /* device scratch for the bf16 operand copies of the tensor-core GEMMs (and split-K partials) */
   size_t scratch_bytes;
-  int gemm_mode;          /* 0: fp32 SIMT everywhere, 1: tensor-core split-bf16 (x3, ~fp32 accuracy), 2: tensor-core plain bf16 */
+  int gemm_mode;          /* 0: fp32 SIMT everywhere, 1: tensor-core split-bf16 (x3, ~fp32 accuracy); any other value: ZEGGS_ERR_ARG */
   int fast_wgrad;         /* 1: weight-gradient products run as ONE bf16 pass (set together with the tensor-core recurrence) */
 } zeggs_ctx;
 
@@ -164,7 +164,6 @@ size_t zeggs_decoder_tc_workspace_bytes(int H, int S, int Z);
 int zeggs_decoder_pack_weights_tc(const zeggs_decoder_fwd_args* a, void* packed, void* stream);
 /* development aid: device buffer [64][32] of int64 receiving CTA 0's per-step phase timestamps (NULL = off) */
 void zeggs_debug_set_tc_trace(void* device_buffer);
-int zeggs_debug_set_tc_gemm_variant(int v);  /* tensor-core GEMM tile variant: -1 automatic (128x256 tiles for one-pass products with N >= 256, fused three-pass), 0 = 128x128 tiles with streamed passes */
 int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* a, void* stream);
 
 /* Backward of zeggs_decoder_window_fwd (the autograd of modules.py:47-162: full BPTT through the GRU stack,

@@ -14,7 +14,7 @@ bf16=True: every MMA operand is rounded to bf16 (round to nearest even) exactly 
 Forward rounding points (decoder_fwd_tc.cu):
   * packed weight slices, __float2bfloat16_rn at :159 / :163 of pack_decoder_tc_kernel: W_ih0[:, :H], W_hh0, W_ih1, W_hh1 (:148-151),
     Mfold (:146) and the root rows W2[0:6] (:147) of the fold chain;
-  * Mfold is rounded after its fp32-grade product (three-pass split-bf16 GEMM with fast_wgrad forced off, :663-665);
+  * Mfold is rounded after its fp32-grade product (three-pass split-bf16 GEMM under a fast_wgrad = 0 copy of the context, :655-657, :679);
   * w2b = bf16(W2) for the batched layer 2 (zeggs_split_bf16, :670; product at :753);
   * activation images a(t) (:483), h0(t) (:526), h1(t) (:566) and the bf16 h1 history of the layer-2 product (:574), plus the images of
     h0(0) / h1(0) that the CellStateEncoder state seeds (image_from_kmajor_kernel :178, launched at :744-745).

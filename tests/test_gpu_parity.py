@@ -1087,28 +1087,28 @@ def test_decoder_single_step_teacher_forced_vs_oracle(dev, H, B):
         assert e1 <= 1e-4 and e2 <= 1e-4
 
 
-def test_two_contexts_do_not_share_state(dev):
-    """The GEMM front end takes its scratch buffer / mode from the caller's zeggs_ctx: two contexts with different modes used
-    alternately on two streams give each its own numerics (fp32 SIMT exact-ish vs plain bf16), with no library-global setter involved."""
+def test_two_fast_wgrad_contexts_do_not_share_state(dev):
+    """The GEMM front end takes its scratch buffer and weight-gradient setting from the caller's zeggs_ctx: two GEMM mode 1 contexts
+    that differ only in fast_wgrad, used alternately on two streams for a weight-gradient layout product (C = A[K,M]^T B[K,N]), give
+    each its own numerics (split-bf16 ~fp32 vs one bf16 pass), with no library-global setter involved."""
     import ctypes as C
     from zeggs_b200 import _lib
     g = torch.Generator().manual_seed(3)
     M, N, K = 256, 384, 512
-    A, B = torch.randn(M, K, generator=g).to(dev), torch.randn(N, K, generator=g).to(dev)
-    ref = A.double() @ B.double().T
+    A, B = torch.randn(K, M, generator=g).to(dev), torch.randn(K, N, generator=g).to(dev)
+    ref = A.double().T @ B.double()
     bufs = [torch.empty(64 << 20, dtype=torch.uint8, device=dev) for _ in range(2)]
-    ctxs = [_lib.Ctx(scratch=bufs[0].data_ptr(), scratch_bytes=bufs[0].numel(), gemm_mode=0, fast_wgrad=0),
-            _lib.Ctx(scratch=bufs[1].data_ptr(), scratch_bytes=bufs[1].numel(), gemm_mode=2, fast_wgrad=0)]
+    ctxs = [_lib.Ctx(scratch=bufs[i].data_ptr(), scratch_bytes=bufs[i].numel(), gemm_mode=1, fast_wgrad=i) for i in (0, 1)]
     streams = [torch.cuda.Stream(dev), torch.cuda.Stream(dev)]
     outs = [torch.empty(M, N, device=dev) for _ in range(2)]
     torch.cuda.synchronize()
     for rep in range(3):
         for i in (0, 1):
-            _lib.check(_lib.lib().zeggs_gemm_f32_ctx(C.addressof(ctxs[i]), 0, M, N, K, A.data_ptr(), K, B.data_ptr(), K, None, outs[i].data_ptr(), N,
+            _lib.check(_lib.lib().zeggs_gemm_f32_ctx(C.addressof(ctxs[i]), 1, M, N, K, A.data_ptr(), M, B.data_ptr(), N, None, outs[i].data_ptr(), N,
                                                      0, 0, streams[i].cuda_stream), "zeggs_gemm_f32_ctx")
     torch.cuda.synchronize()
     e0 = float((outs[0].double() - ref).abs().max() / ref.abs().max())
     e1 = float((outs[1].double() - ref).abs().max() / ref.abs().max())
-    print(f"  ctx0 (fp32 SIMT) rel err {e0:.2e}; ctx1 (plain bf16 tensor cores) rel err {e1:.2e}")
+    print(f"  ctx0 (split-bf16, fast_wgrad 0) rel err {e0:.2e}; ctx1 (one bf16 pass, fast_wgrad 1) rel err {e1:.2e}")
     assert e0 <= 2e-5 and 1e-4 <= e1 <= 2e-2
 

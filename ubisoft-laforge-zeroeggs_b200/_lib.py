@@ -153,7 +153,6 @@ SYMBOLS = [
     ("zeggs_decoder_tc_workspace_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_decoder_pack_weights_tc", C.c_int, [C.POINTER(DecoderFwdArgs), C.c_void_p, C.c_void_p]),
     ("zeggs_debug_set_tc_trace", None, [C.c_void_p]),
-    ("zeggs_debug_set_tc_gemm_variant", C.c_int, [C.c_int]),
     ("zeggs_decoder_packed_bwd_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_decoder_pack_weights_bwd", C.c_int, [C.POINTER(DecoderFwdArgs), C.c_void_p, C.c_void_p]),
     ("zeggs_decoder_bwd_workspace_bytes", C.c_size_t, [C.c_int] * 5),

@@ -85,7 +85,7 @@ extern "C" int zeggs_timing_read(const char* name, double* total_ms, int* count)
 }
 
 extern "C" const char* zeggs_last_error(void) { return zeggs::get_error(); }
-extern "C" int zeggs_version(void) { return 101; }
+extern "C" int zeggs_version(void) { return 102; }
 extern "C" long long zeggs_launch_count(void) { return zeggs::g_launches.load(); }
 
 // sizeof of every args struct of include/zeggs_b200.h by its C name (0 = unknown): lets a binding in another language check at load

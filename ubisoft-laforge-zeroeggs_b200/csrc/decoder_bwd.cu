@@ -602,7 +602,7 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
   // in GEMM mode 1 for ~fp32 accuracy), the SIMT k-major kernels otherwise
   const bool want_lo = gemm_mode() == 1;
   const WgradHists hs = wgrad_hists(a, b, g, w, bw, want_lo);
-  if (gemm_mode() != 0 && scratch_base() != nullptr && hs.bytes <= scratch_bytes()) {
+  if (gemm_mode() == 1 && scratch_base() != nullptr && hs.bytes <= scratch_bytes()) {
     for (int i = 0; i < NHIST; ++i) if ((rc = split_hist(hs, i, stream))) return rc;
     if ((rc = wgrad_gemms(a, b, g, hs, want_lo, hs.end, stream))) return rc;
   } else {

@@ -596,8 +596,8 @@ int decoder_window_bwd_tc(const zeggs_decoder_fwd_args& a, const zeggs_decoder_b
   ZCHECK_SUPPORTED(tc_hidden_ok(H), "decoder bwd tc: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", H);
   ZCHECK_ARG(g.nbt == 1 && bg.n4b == 1, "decoder bwd tc engine needs B <= 32 (got B=%d)", a.B);
   ZCHECK_ARG(b.workspace_tc, "decoder bwd tc: workspace_tc missing");
-  ZCHECK_ARG(gemm_mode() != 0 && scratch_base() != nullptr,
-             "decoder bwd tc: needs the tensor-core GEMM front end (a zeggs_ctx with scratch, gemm mode 1 or 2)");
+  ZCHECK_ARG(gemm_mode() == 1 && scratch_base() != nullptr,
+             "decoder bwd tc: needs the tensor-core GEMM front end (a zeggs_ctx with scratch, gemm mode 1)");
   // PRE[(b,t)][j] = sum_n W2[n][j] out_std[n] dY[b][t][n]: the layer-2 adjoint of the external gradient for every frame at once,
   // operands and result at the scratch base for the duration of the recurrence
   const int ldy = round_up(P_OUT, 8);

@@ -32,7 +32,6 @@ struct CtxScope {
   ~CtxScope() { if (active) swap_ctx(old); }
 };
 int gemm_mode();
-int set_fast_wgrad_internal(int on);   // returns the previous setting
 char* scratch_base();
 size_t scratch_bytes();
 int split_hist_launch(const float* x, long long slot_stride, int S, int R, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t stream,

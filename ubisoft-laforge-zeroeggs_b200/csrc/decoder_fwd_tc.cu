@@ -651,7 +651,10 @@ extern "C" size_t zeggs_decoder_tc_workspace_bytes(int H, int S, int Z) {
   return make_tcws(nullptr, g).bytes;
 }
 extern "C" int zeggs_decoder_pack_weights_tc(const zeggs_decoder_fwd_args* a, void* packed, void* stream_) {
-  CtxScope ctx_scope(a ? a->ctx : nullptr);
+  // the fold matrix is the one layout-1 product that is not a weight gradient: it always gets the fp32-grade three-pass GEMM
+  zeggs_ctx fold_ctx = {};
+  if (a && a->ctx) { fold_ctx = *a->ctx; fold_ctx.fast_wgrad = 0; }
+  CtxScope ctx_scope(a && a->ctx ? &fold_ctx : nullptr);
   ZCHECK_ARG(a && packed, "decoder tc pack: bad arguments");
   ZCHECK_SUPPORTED(tc_hidden_ok(a->H), "decoder tc pack: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", a->H);
   ZCHECK_ARG(a->in_mean && a->in_std && a->out_mean && a->out_std, "decoder tc pack: normalisation statistics missing");
@@ -673,9 +676,7 @@ extern "C" int zeggs_decoder_pack_weights_tc(const zeggs_decoder_fwd_args* a, vo
   count_launch();
   ZCHECK_LAUNCH();
   // Mfold[4H][H] = WxDt^T [4H x 1131] . W2 [1131 x H]     (fp32-grade: split-bf16 tensor-core GEMM when a scratch buffer is set)
-  const int fw = set_fast_wgrad_internal(0);       // the fold matrix is a weight product: always the fp32-grade 3-pass GEMM
   int rc = gemm_f32_auto(1, 4 * H, H, P_OUT, wxdt, 4 * H, a->W2, H, nullptr, mfold, H, 0, 0, stream);
-  set_fast_wgrad_internal(fw);
   if (rc) return rc;
   pack_decoder_tc_kernel<<<592, 256, 0, stream>>>(g, tg, mfold, a->W_ih0, a->W_hh0, a->W_ih1, a->W_hh1, a->W2, base);
   count_launch();

@@ -3,7 +3,7 @@
 // One 128 x BN output tile per CTA; BLOCK_K = 64 bf16 (one 128-byte swizzle atom row).
 // Warp roles (288 threads): warps 0..3 and 4..7 = two consumer warpgroups (rows 0..63 / 64..127 of the tile, accumulators in
 // registers, wgmma.m64n128k16 per 128 columns), warp 8 = TMA producer.
-// `passes` > 1 implements the split-bf16 ("bf16x3") scheme: x = hi + lo with hi = bf16(x),
+// Three passes implement the split-bf16 ("bf16x3") scheme: x = hi + lo with hi = bf16(x),
 // lo = bf16(x - hi); passes (A_hi,B_hi), (A_lo,B_hi), (A_hi,B_lo) accumulate into the same accumulator,
 // recovering ~fp32 product accuracy at 3x the tensor work.
 #include <cuda.h>
@@ -22,15 +22,14 @@ struct TcGemmMaps {
   CUtensorMap b[2];
 };
 
-// Two variants cut the operand bytes per MMA:
-//   BN = 256 (one-pass products with N >= 256): A 16 KB + B 32 KB per stage, each A byte feeds twice the columns;
-//   FUSE (the split-bf16 three-pass scheme): A_hi, A_lo, B_hi, B_lo of a k-block are staged ONCE (64 KB) and the three products
-//   hi*hi, lo*hi, hi*lo issued back to back from that stage instead of streaming the operands three times.
+// One-pass products stage A and B per k-block; BN = 256 (N >= 256) holds A 16 KB + B 32 KB per stage, so each A byte feeds
+// twice the columns.  FUSE is the split-bf16 three-pass scheme: A_hi, A_lo, B_hi, B_lo of a k-block are staged ONCE (64 KB) and
+// the three products hi*hi, lo*hi, hi*lo issued back to back from that stage.
 // Epilogue: the accumulators go through a padded shared-memory tile (the pipeline stages are dead once both warpgroups have
 // passed the final wait) so that the global accesses are row-contiguous, read-modify-write of C included.
 template <int BN, int STAGES, bool FUSE>
 __global__ void __launch_bounds__(TG_THREADS, 1)
-tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K, int passes,
+tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K,
                const float* __restrict__ bias, float* __restrict__ C, int ldc, int act, int accumulate,
                float* __restrict__ part, int kb_per_split) {
   constexpr int B_BYTES = BN * TG_BK * 2;
@@ -52,11 +51,9 @@ tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K, int
   // split-K: blockIdx.z owns k-blocks [kb0, kb0 + kblocks); its raw fp32 tile goes to part[z][M][N] (reduced afterwards)
   const int kb0 = blockIdx.z * kb_per_split;
   const int kblocks = min(kb_per_split, ceil_div(K, TG_BK) - kb0);
-  // unfused pass order: (A0,B0), (A1,B0), (A0,B1)
-  const int total = kblocks * ((FUSE || passes == 1) ? 1 : 3);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < (passes == 1 ? 1 : 2); ++i) { tma_prefetch_desc(&maps.a[i]); tma_prefetch_desc(&maps.b[i]); }
+    for (int i = 0; i < NOP; ++i) { tma_prefetch_desc(&maps.a[i]); tma_prefetch_desc(&maps.b[i]); }
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // empty: one arrival per consumer warp
     fence_mbar_init();
   }
@@ -64,23 +61,15 @@ tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K, int
 
   if (warp == 8) {
     if (lane == 0) {
-      for (int it = 0; it < total; ++it) {
-        const int s = it % STAGES, ph = (it / STAGES) & 1;
+      for (int it = 0; it < kblocks; ++it) {
+        const int s = it % STAGES, ph = (it / STAGES) & 1, kb = kb0 + it;
         mbar_wait(&empty[s], ph ^ 1);
+        mbar_arrive_expect_tx(&full[s], STAGE_A + STAGE_B);
+        tma_load_2d(sA + s * STAGE_A, &maps.a[0], &full[s], kb * TG_BK, m0);
+        tma_load_2d(sB + s * STAGE_B, &maps.b[0], &full[s], kb * TG_BK, n0);
         if (FUSE) {
-          const int kb = kb0 + it;
-          mbar_arrive_expect_tx(&full[s], STAGE_A + STAGE_B);
-          tma_load_2d(sA + s * STAGE_A, &maps.a[0], &full[s], kb * TG_BK, m0);
-          tma_load_2d(sB + s * STAGE_B, &maps.b[0], &full[s], kb * TG_BK, n0);
           tma_load_2d(sA + s * STAGE_A + TG_A_BYTES, &maps.a[1], &full[s], kb * TG_BK, m0);
           tma_load_2d(sB + s * STAGE_B + B_BYTES, &maps.b[1], &full[s], kb * TG_BK, n0);
-        } else {
-          const int p = it / kblocks, kb = kb0 + it - p * kblocks;
-          const CUtensorMap* ma = &maps.a[p == 1 ? 1 : 0];
-          const CUtensorMap* mb = &maps.b[p == 2 ? 1 : 0];
-          mbar_arrive_expect_tx(&full[s], STAGE_A + STAGE_B);
-          tma_load_2d(sA + s * STAGE_A, ma, &full[s], kb * TG_BK, m0);
-          tma_load_2d(sB + s * STAGE_B, mb, &full[s], kb * TG_BK, n0);
         }
       }
     }
@@ -90,7 +79,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K, int
   const int wg = warp >> 2;
   float d[NJ][64];
   int prev = 0;
-  for (int it = 0; it < total; ++it) {
+  for (int it = 0; it < kblocks; ++it) {
     const int s = it % STAGES, ph = (it / STAGES) & 1;
     mbar_wait(&full[s], ph);
     const uint64_t da = make_smem_desc_sw128(sA + s * STAGE_A + wg * (64 * 128));
@@ -332,48 +321,27 @@ int num_sms() {
   return n;
 }
 
-// experiment knob: 0 forces the round-1 kernel shape (128x128 tiles, passes streamed one after the other), -1 = automatic
-static int g_tc_gemm_variant = -1;
-extern "C" int zeggs_debug_set_tc_gemm_variant(int v) { g_tc_gemm_variant = v; return ZEGGS_OK; }
-static int tc_gemm_variant_override() { return g_tc_gemm_variant; }
-
 int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, int lda,
                    const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, const float* bias,
                    float* C, int ldc, int act, int accumulate, cudaStream_t stream, float* splitk_ws, size_t splitk_ws_bytes) {
   ZCHECK_ARG(M > 0 && N > 0 && K > 0 && A_hi && B_hi && C, "tc_gemm: bad arguments");
   ZCHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "tc_gemm: leading dimensions must be multiples of 8 bf16 (16 B)");
   ZCHECK_ARG(((uintptr_t)A_hi & 15) == 0 && ((uintptr_t)B_hi & 15) == 0, "tc_gemm: operands must be 16-byte aligned");
-  const int passes = (A_lo && B_lo) ? 3 : 1;
-  // variant: 0 = 128x128 tiles, 4 stages;  1 = 128x256 tiles (one-pass products, N >= 256);  2 = fused three-pass, 128x128, 3 stages
-  const int forced = tc_gemm_variant_override();
-  auto plan = [&](int bm, int bn, int* splits_out) {
-    const int tiles = ceil_div(N, bn) * ceil_div(M, bm), kblocks = ceil_div(K, TG_BK);
-    int sp = 1;
-    if (splitk_ws && tiles <= num_sms() / 2 && kblocks >= 8) {
-      sp = std::min(std::max(1, num_sms() / tiles), kblocks / 2);
-      const size_t per = (size_t)M * N * sizeof(float);
-      if ((size_t)sp * per > splitk_ws_bytes) sp = (int)(splitk_ws_bytes / per);
-      if (sp < 1) sp = 1;
-    }
-    *splits_out = sp;
-    return sp;
-  };
-  int variant = passes == 3 ? 2 : (N >= 256 ? 1 : 0);
-  if (forced == 0) variant = 0;
-  else if (forced == 1 && passes == 1 && N >= 256) variant = 1;
-  const int BN = variant == 1 ? 256 : 128;
-  const int BMT = TG_BM;
+  // tiles: split-bf16 (hi and lo of both operands) -> fused three passes, 128x128, 3 stages; one pass -> 128x256 when N >= 256,
+  // 128x128 otherwise, 4 stages
+  const bool fused = A_lo && B_lo;
+  const int BN = !fused && N >= 256 ? 256 : 128;
   TcGemmMaps maps;
   memset(&maps, 0, sizeof(maps));
   int rc;
-  if ((rc = encode_map(&maps.a[0], A_hi, M, K, lda, BMT))) return rc;
+  if ((rc = encode_map(&maps.a[0], A_hi, M, K, lda, TG_BM))) return rc;
   if ((rc = encode_map(&maps.b[0], B_hi, N, K, ldb, BN))) return rc;
-  if (passes == 3) {
-    if ((rc = encode_map(&maps.a[1], A_lo, M, K, lda, BMT))) return rc;
+  if (fused) {
+    if ((rc = encode_map(&maps.a[1], A_lo, M, K, lda, TG_BM))) return rc;
     if ((rc = encode_map(&maps.b[1], B_lo, N, K, ldb, BN))) return rc;
   }
   auto smem_of = [](int bm, int bn, int stages, int nop) { return (size_t)1024 + (size_t)stages * nop * (bm * TG_BK * 2 + bn * TG_BK * 2) + (2 * stages + 1) * 8 + 16; };
-  const size_t smem = variant == 1 ? smem_of(128, 256, 4, 1) : variant == 2 ? smem_of(128, 128, 3, 2) : smem_of(128, 128, 4, 1);
+  const size_t smem = fused ? smem_of(128, 128, 3, 2) : BN == 256 ? smem_of(128, 256, 4, 1) : smem_of(128, 128, 4, 1);
   static bool attr_set = false;     // one device per process (one rank per GPU): set once, not on every launch
   if (!attr_set) {
     ZCHECK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<128, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 128, 4, 1)));
@@ -381,26 +349,28 @@ int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bf
     ZCHECK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<128, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 128, 3, 2)));
     attr_set = true;
   }
-  dim3 grid(ceil_div(N, BN), ceil_div(M, BMT));
-  // split-K when the output has too few tiles to fill the SMs and the contraction is long
-  const int kblocks = ceil_div(K, TG_BK);
+  // split-K when the output has too few tiles to fill the SMs and the contraction is long: blockIdx.z writes its raw partial tile to
+  // splitk_ws, and splitk_reduce_kernel sums them in a fixed order and applies the epilogue
+  const int tiles = ceil_div(N, BN) * ceil_div(M, TG_BM), kblocks = ceil_div(K, TG_BK);
   int splits = 1;
-  plan(BMT, BN, &splits);
-  auto launch = [&](const float* bias_, int act_, int acc_, float* part, int kbs) {
-    if (variant == 1) tc_gemm_kernel<256, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, passes, bias_, C, ldc, act_, acc_, part, kbs);
-    else if (variant == 2) tc_gemm_kernel<128, 3, true><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, passes, bias_, C, ldc, act_, acc_, part, kbs);
-    else tc_gemm_kernel<128, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, passes, bias_, C, ldc, act_, acc_, part, kbs);
-    count_launch();
-  };
-  if (splits <= 1) {
-    launch(bias, act, accumulate, nullptr, kblocks);
-  } else {
-    const int kbs = ceil_div(kblocks, splits);
-    splits = ceil_div(kblocks, kbs);                      // every z gets at least one k-block
-    grid.z = splits;
-    launch(nullptr, 0, 0, splitk_ws, kbs);
+  if (splitk_ws && tiles <= num_sms() / 2 && kblocks >= 8) {
+    splits = std::min(std::max(1, num_sms() / tiles), kblocks / 2);
+    const size_t per = (size_t)M * N * sizeof(float);
+    if ((size_t)splits * per > splitk_ws_bytes) splits = (int)(splitk_ws_bytes / per);
+    splits = std::max(splits, 1);
+  }
+  const int kbs = ceil_div(kblocks, splits);
+  splits = ceil_div(kblocks, kbs);                        // every z gets at least one k-block
+  float* const part = splits > 1 ? splitk_ws : nullptr;
+  const dim3 grid(ceil_div(N, BN), ceil_div(M, TG_BM), splits);
+  // with `part` set the kernel stores the raw tile and leaves bias, act and accumulate to the reduction
+  if (fused) tc_gemm_kernel<128, 3, true><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs);
+  else if (BN == 256) tc_gemm_kernel<256, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs);
+  else tc_gemm_kernel<128, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs);
+  count_launch();
+  if (part) {
     const size_t total = (size_t)M * N;
-    splitk_reduce_kernel<<<(int)std::min<size_t>(1184, (total + 255) / 256), 256, 0, stream>>>(splitk_ws, splits, M, N, bias, C, ldc, act, accumulate);
+    splitk_reduce_kernel<<<(int)std::min<size_t>(1184, (total + 255) / 256), 256, 0, stream>>>(part, splits, M, N, bias, C, ldc, act, accumulate);
     count_launch();
   }
   ZCHECK_LAUNCH();
@@ -420,10 +390,7 @@ int split_t_launch(const float* x, int rows, int cols, int ld_in, __nv_bfloat16*
 // im2col path.
 static const zeggs_ctx k_no_ctx = {nullptr, 0, 1, 0};
 static thread_local const zeggs_ctx* tl_ctx = &k_no_ctx;
-static thread_local int tl_fast_wgrad_override = -1;
 const zeggs_ctx* swap_ctx(const zeggs_ctx* c) { const zeggs_ctx* old = tl_ctx; tl_ctx = c; return old; }
-static int fast_wgrad() { return tl_fast_wgrad_override >= 0 ? tl_fast_wgrad_override : tl_ctx->fast_wgrad; }
-int set_fast_wgrad_internal(int on) { const int old = tl_fast_wgrad_override; tl_fast_wgrad_override = on; return old; }
 int gemm_mode() { return tl_ctx->gemm_mode; }
 char* scratch_base() { return (char*)tl_ctx->scratch; }
 size_t scratch_bytes() { return tl_ctx->scratch_bytes; }
@@ -436,37 +403,58 @@ int split_hist_launch(const float* x, long long slot_stride, int S, int R, __nv_
   return ZEGGS_OK;
 }
 
+// bf16 operands of one tensor-core product, carved from the scratch buffer in this order: Ah [rows_a][Kp], Bh [rows_b][Kp], then
+// (three-pass products only) Al, Bl, each rounded up to 256 bytes.  The split-K partial tiles get the rest of the buffer, so the
+// carve fixes the split count and with it the summation order.
+struct TcOperands {
+  __nv_bfloat16 *Ah, *Bh, *Al, *Bl;   // Al = Bl = nullptr for a one-pass product
+  float* ws;
+  size_t ws_bytes;
+};
+
+// The rule for which arithmetic a product of the front end gets, given the active context.  A product runs on the tensor cores
+// when the context is in GEMM mode 1, has scratch, the product has at least 4e6 multiply-adds and its operand copies fit the
+// scratch; it is then split-bf16 (three passes, ~fp32 accuracy), or one bf16 pass for a weight gradient when the context sets
+// fast_wgrad.  -> ZEGGS_OK with *op carved; ZEGGS_CONV_NOT_TAKEN when the product belongs on the SIMT path; ZEGGS_ERR_ARG for a
+// GEMM mode other than 0 or 1.
+static int plan_tc_operands(int rows_a, int rows_b, int Kp, double macs, bool wgrad, TcOperands* op) {
+  const zeggs_ctx& c = *tl_ctx;
+  ZCHECK_ARG(c.gemm_mode == 0 || c.gemm_mode == 1, "zeggs_ctx.gemm_mode must be 0 (fp32 SIMT) or 1 (tensor-core split-bf16), got %d",
+             c.gemm_mode);
+  char* const base = (char*)c.scratch;
+  if (c.gemm_mode == 0 || base == nullptr || macs < 4.0e6) return ZEGGS_CONV_NOT_TAKEN;
+  const bool lo = !(wgrad && c.fast_wgrad);
+  char* p = base;
+  auto take = [&](int rows) { __nv_bfloat16* r = (__nv_bfloat16*)p; p += ((size_t)rows * Kp * 2 + 255) / 256 * 256; return r; };
+  op->Ah = take(rows_a);
+  op->Bh = take(rows_b);
+  op->Al = lo ? take(rows_a) : nullptr;
+  op->Bl = lo ? take(rows_b) : nullptr;
+  p = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255);
+  if ((size_t)(p - base) > c.scratch_bytes) return ZEGGS_CONV_NOT_TAKEN;
+  op->ws = (float*)p;
+  op->ws_bytes = c.scratch_bytes - (size_t)(p - base);
+  return ZEGGS_OK;
+}
+
 // mode 0: C = act(A[M,K] B[N,K]^T + bias);  1: C = A[K,M]^T B[K,N];  2: C = A[M,K] B[K,N]   (all fp32, row-major)
-// Large products go through the tensor cores (operands split to bf16 hi/lo in the scratch buffer); small ones, or no scratch,
-// use the fp32 SIMT kernel.
+// Mode 1 is the layout of the weight gradients.  plan_tc_operands picks the tensor cores or the fp32 SIMT kernel.
 int gemm_f32_auto(int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb, const float* bias,
                   float* C, int ldc, int act, int accumulate, cudaStream_t stream) {
   const int Kp = round_up(K, 8);
-  const size_t elems = (size_t)(M + N) * Kp;
-  char* const sbase = scratch_base();
-  const size_t sbytes = scratch_bytes();
-  const int gmode = gemm_mode();
-  const bool want_lo = gmode == 1 && !(mode == 1 && fast_wgrad());
-  const size_t need = elems * 2 * (want_lo ? 2 : 1) + 1024;
-  if (gmode == 0 || sbase == nullptr || need > sbytes || (double)M * N * K < 4.0e6)
-    return sgemm_launch(mode, M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, stream);
-  char* p = sbase;
-  auto take = [&](size_t n) { __nv_bfloat16* r = (__nv_bfloat16*)p; p += ((n * 2 + 255) / 256) * 256; return r; };
-  __nv_bfloat16* Ah = take((size_t)M * Kp); __nv_bfloat16* Bh = take((size_t)N * Kp);
-  __nv_bfloat16* Al = want_lo ? take((size_t)M * Kp) : nullptr; __nv_bfloat16* Bl = want_lo ? take((size_t)N * Kp) : nullptr;
-  if ((size_t)(p - sbase) > sbytes)
-    return sgemm_launch(mode, M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, stream);
+  TcOperands op;
+  const int rc = plan_tc_operands(M, N, Kp, (double)M * N * K, mode == 1, &op);
+  if (rc == ZEGGS_CONV_NOT_TAKEN) return sgemm_launch(mode, M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, stream);
+  if (rc) return rc;
   const dim3 tb(32, 8);
-  if (mode == 1) split_bf16_t_kernel<<<dim3(ceil_div(M, 32), ceil_div(Kp, 32)), tb, 0, stream>>>(A, K, M, lda, Ah, Al, Kp);
-  else split_bf16_kernel<<<592, 256, 0, stream>>>(A, M, K, lda, Ah, Al, Kp);
+  if (mode == 1) split_bf16_t_kernel<<<dim3(ceil_div(M, 32), ceil_div(Kp, 32)), tb, 0, stream>>>(A, K, M, lda, op.Ah, op.Al, Kp);
+  else split_bf16_kernel<<<592, 256, 0, stream>>>(A, M, K, lda, op.Ah, op.Al, Kp);
   count_launch();
-  if (mode == 0) split_bf16_kernel<<<592, 256, 0, stream>>>(B, N, K, ldb, Bh, Bl, Kp);
-  else split_bf16_t_kernel<<<dim3(ceil_div(N, 32), ceil_div(Kp, 32)), tb, 0, stream>>>(B, K, N, ldb, Bh, Bl, Kp);
+  if (mode == 0) split_bf16_kernel<<<592, 256, 0, stream>>>(B, N, K, ldb, op.Bh, op.Bl, Kp);
+  else split_bf16_t_kernel<<<dim3(ceil_div(N, 32), ceil_div(Kp, 32)), tb, 0, stream>>>(B, K, N, ldb, op.Bh, op.Bl, Kp);
   count_launch();
   ZCHECK_LAUNCH();
-  p = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255);
-  return tc_gemm_launch(M, N, K, Ah, Al, Kp, Bh, Bl, Kp, bias, C, ldc, act, accumulate, stream, (float*)p,
-                        (size_t)(sbase + sbytes - p));
+  return tc_gemm_launch(M, N, K, op.Ah, op.Al, Kp, op.Bh, op.Bl, Kp, bias, C, ldc, act, accumulate, stream, op.ws, op.ws_bytes);
 }
 
 // ------------------------------------------------------------------ convolution operands without a materialised im2col matrix
@@ -550,48 +538,30 @@ __global__ void im2col_split_t_kernel(const float* __restrict__ x, int B, int T,
 int conv_gemm_fwd(const float* x, int B, int T, int C, int k, int pad, int replicate, const float* W, const float* bias, float* y, int N,
                   int act, cudaStream_t stream) {
   const int M = B * T, K = C * k, Kp = round_up(K, 8);
-  char* const sbase = scratch_base();
-  const size_t sbytes = scratch_bytes();
-  const int gmode = gemm_mode();
-  const bool want_lo = gmode == 1;
-  const size_t need = (size_t)(M + N) * Kp * 2 * (want_lo ? 2 : 1) + 2048;
-  if (gmode == 0 || sbase == nullptr || need > sbytes || (double)M * N * K < 4.0e6) return ZEGGS_CONV_NOT_TAKEN;
-  char* p = sbase;
-  auto take = [&](size_t n) { __nv_bfloat16* r = (__nv_bfloat16*)p; p += ((n * 2 + 255) / 256) * 256; return r; };
-  __nv_bfloat16* Ah = take((size_t)M * Kp); __nv_bfloat16* Bh = take((size_t)N * Kp);
-  __nv_bfloat16* Al = want_lo ? take((size_t)M * Kp) : nullptr; __nv_bfloat16* Bl = want_lo ? take((size_t)N * Kp) : nullptr;
-  if ((size_t)(p - sbase) > sbytes) return ZEGGS_CONV_NOT_TAKEN;
-  im2col_split_kernel<<<std::min(M, num_sms() * 16), 256, 0, stream>>>(x, B, T, C, k, pad, replicate, Ah, Al, Kp);
+  TcOperands op;
+  const int rc = plan_tc_operands(M, N, Kp, (double)M * N * K, false, &op);
+  if (rc) return rc;
+  im2col_split_kernel<<<std::min(M, num_sms() * 16), 256, 0, stream>>>(x, B, T, C, k, pad, replicate, op.Ah, op.Al, Kp);
   count_launch();
-  split_bf16_kernel<<<592, 256, 0, stream>>>(W, N, K, K, Bh, Bl, Kp);
+  split_bf16_kernel<<<592, 256, 0, stream>>>(W, N, K, K, op.Bh, op.Bl, Kp);
   count_launch();
   ZCHECK_LAUNCH();
-  p = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255);
-  return tc_gemm_launch(M, N, K, Ah, Al, Kp, Bh, Bl, Kp, bias, y, N, act, 0, stream, (float*)p, (size_t)(sbase + sbytes - p));
+  return tc_gemm_launch(M, N, K, op.Ah, op.Al, Kp, op.Bh, op.Bl, Kp, bias, y, N, act, 0, stream, op.ws, op.ws_bytes);
 }
 
 // dW[n][c*k+kk] = sum_{(b,t)} dpre[(b,t)][n] x[b][t+kk-pad][c]
 int conv_gemm_wgrad(const float* dpre, int N, const float* x, int B, int T, int C, int k, int pad, int replicate, float* dW, cudaStream_t stream) {
   const int M = B * T, K = C * k, Mp = round_up(M, 8);
-  char* const sbase = scratch_base();
-  const size_t sbytes = scratch_bytes();
-  const int gmode = gemm_mode();
-  const bool want_lo = gmode == 1 && !fast_wgrad();
-  const size_t need = (size_t)(N + K) * Mp * 2 * (want_lo ? 2 : 1) + 2048;
-  if (gmode == 0 || sbase == nullptr || need > sbytes || (double)M * N * K < 4.0e6) return ZEGGS_CONV_NOT_TAKEN;
-  char* p = sbase;
-  auto take = [&](size_t n) { __nv_bfloat16* r = (__nv_bfloat16*)p; p += ((n * 2 + 255) / 256) * 256; return r; };
-  __nv_bfloat16* Ah = take((size_t)N * Mp); __nv_bfloat16* Bh = take((size_t)K * Mp);
-  __nv_bfloat16* Al = want_lo ? take((size_t)N * Mp) : nullptr; __nv_bfloat16* Bl = want_lo ? take((size_t)K * Mp) : nullptr;
-  if ((size_t)(p - sbase) > sbytes) return ZEGGS_CONV_NOT_TAKEN;
+  TcOperands op;
+  const int rc = plan_tc_operands(N, K, Mp, (double)M * N * K, true, &op);
+  if (rc) return rc;
   const dim3 tb(32, 8);
-  split_bf16_t_kernel<<<dim3(ceil_div(N, 32), ceil_div(Mp, 32)), tb, 0, stream>>>(dpre, M, N, N, Ah, Al, Mp);
+  split_bf16_t_kernel<<<dim3(ceil_div(N, 32), ceil_div(Mp, 32)), tb, 0, stream>>>(dpre, M, N, N, op.Ah, op.Al, Mp);
   count_launch();
-  im2col_split_t_kernel<<<dim3(ceil_div(C, 32), ceil_div(Mp, 128), k), tb, 0, stream>>>(x, B, T, C, k, pad, replicate, Bh, Bl, Mp);
+  im2col_split_t_kernel<<<dim3(ceil_div(C, 32), ceil_div(Mp, 128), k), tb, 0, stream>>>(x, B, T, C, k, pad, replicate, op.Bh, op.Bl, Mp);
   count_launch();
   ZCHECK_LAUNCH();
-  p = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255);
-  return tc_gemm_launch(N, K, M, Ah, Al, Mp, Bh, Bl, Mp, nullptr, dW, K, 0, 0, stream, (float*)p, (size_t)(sbase + sbytes - p));
+  return tc_gemm_launch(N, K, M, op.Ah, op.Al, Mp, op.Bh, op.Bl, Mp, nullptr, dW, K, 0, 0, stream, op.ws, op.ws_bytes);
 }
 
 extern "C" int zeggs_gemm_f32_ctx(const zeggs_ctx* ctx, int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb,

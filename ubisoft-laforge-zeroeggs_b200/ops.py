@@ -36,24 +36,17 @@ WS = _Workspace()
 
 _scratch = {}
 _ctx = {}
-GEMM_MODE = 1          # 0: fp32 SIMT everywhere, 1: tensor-core split-bf16 (~fp32 accuracy), 2: tensor-core plain bf16
-# experiment knob: with the tensor-core recurrence engine selected, run the batched GEMMs (encoders, hoisted terms, fold matrix) as ONE
-# bf16 pass instead of the 3-pass split-bf16 scheme
-TC_GEMM_BF16 = __import__("os").environ.get("ZEGGS_TC_GEMM_BF16", "0") == "1"
-
-
-def _effective_gemm_mode():
-    return 2 if (TC_GEMM_BF16 and GEMM_MODE == 1 and DECODER_ENGINE != "fp32") else GEMM_MODE
+GEMM_MODE = 1          # 0: fp32 SIMT everywhere, 1: tensor-core split-bf16 (~fp32 accuracy)
 
 
 def set_gemm_mode(mode):
     """GEMM engine of the batched (non-recurrent) products for subsequent calls from this process."""
     global GEMM_MODE
-    if mode not in (0, 1, 2):
-        raise _lib.ZeggsError("gemm mode must be 0 (fp32 SIMT), 1 (tensor-core bf16x3) or 2 (tensor-core bf16)")
+    if mode not in (0, 1):
+        raise _lib.ZeggsError("gemm mode must be 0 (fp32 SIMT) or 1 (tensor-core bf16x3)")
     GEMM_MODE = mode
     for c in _ctx.values():
-        c.gemm_mode = _effective_gemm_mode()
+        c.gemm_mode = mode
 
 
 # Lanes: calls that run CONCURRENTLY on different CUDA streams (the two encoders next to each other, the encoders' backward next to the
@@ -91,7 +84,7 @@ def ensure_scratch(dev):
         mb = int(os.environ.get("ZEGGS_SCRATCH_MB", "1536")) if ln == "main" else int(os.environ.get("ZEGGS_LANE_SCRATCH_MB", "768"))
         buf = torch.empty(mb << 20, dtype=torch.uint8, device=dev)
         _scratch[key] = buf
-        _ctx[key] = _lib.Ctx(scratch=buf.data_ptr(), scratch_bytes=buf.numel(), gemm_mode=_effective_gemm_mode(),
+        _ctx[key] = _lib.Ctx(scratch=buf.data_ptr(), scratch_bytes=buf.numel(), gemm_mode=GEMM_MODE,
                              fast_wgrad=0 if DECODER_ENGINE == "fp32" else 1)
     return _scratch[key]
 
@@ -125,7 +118,6 @@ def set_decoder_engine(name):
     # the tensor-core engine's weight gradients are single-pass bf16: the encoders' weight-gradient GEMMs follow it
     for c in _ctx.values():
         c.fast_wgrad = 0 if name == "fp32" else 1
-        c.gemm_mode = _effective_gemm_mode()
 
 
 def resolve_engine(H, S, Z):
