@@ -892,8 +892,9 @@ def test_graph_replayed_train_steps_match_eager_launches(dev, decoder_engine):
 
 def test_concurrent_lanes_match_single_stream_step(dev, decoder_engine, monkeypatch):
     """TrainStep with the concurrent lanes (encoders side by side; encoders' backward next to the decoder's phase-2 weight gradients,
-    each lane with its own stream and GEMM scratch) against the same steps issued on ONE stream with the one-call decoder backward:
-    every kernel is deterministic and the lanes only reorder independent work, so losses and parameters must be identical."""
+    each lane with its own stream and GEMM scratch) against the same calls issued in the same order on ONE stream: every kernel is
+    deterministic and the lanes only reorder independent work, so losses and parameters must be identical.  Both runs use the
+    two-phase decoder backward; test_two_phase_decoder_backward_matches_one_call pins it to the one-call form."""
     from zeggs_b200 import modules, synth
     from zeggs_b200.train import TrainStep
     decoder_engine("tc")
@@ -915,6 +916,38 @@ def test_concurrent_lanes_match_single_stream_step(dev, decoder_engine, monkeypa
     print("  lanes  losses", res["1"][0]); print("  serial losses", res["0"][0])
     assert res["1"][0] == res["0"][0]
     assert float((res["1"][1] - res["0"][1]).abs().max()) == 0.0
+
+
+@pytest.mark.parametrize("engine,H", [("tc", 384), ("fp32", 128)])
+def test_two_phase_decoder_backward_matches_one_call(dev, decoder_engine, engine, H):
+    """ops.decoder_window_backward in one call and in two phases (split=True, then finish()) on the same saved forward: every decoder
+    parameter gradient, dSpeech and dStyle bitwise equal, on both engines."""
+    from zeggs_b200 import ops, synth
+    from zeggs_b200.train import POSE_KEYS, pack_pose
+    decoder_engine(engine)
+    B, T = 4, 16
+    P = synth.make_params(H=H, seed=82, with_style=False)
+    dec = make_decoder(P, H, device=dev).train()
+    win = tt(synth.make_pose_windows(B, T, seed=82), dev)
+    rs = np.random.RandomState(82)
+    randn = lambda *shape: torch.from_numpy(rs.randn(*shape).astype(np.float32)).to(dev)
+    st = stats_tensors(dev)
+    stats = [st[k] for k in ("anim_input_mean", "anim_input_std", "anim_output_mean", "anim_output_std")]
+    W = [win[k] for k in POSE_KEYS]
+    WY = pack_pose(*W[2:])
+    Y, rp, rq, state = ops.decoder_window_forward(dec, W[0][:, 0], W[1][:, 0], WY[:, 0], win["gaze_pos"], 0.5 * randn(B, T, 64),
+                                                  randn(B, T, 64), stats, st["dt"], save=True)
+    assert state[0].engine == (1 if engine == "tc" else 0)
+    cot = (randn(*Y.shape), randn(*rp.shape), randn(*rq.shape))
+    grads, dSpeech, dStyle = ops.decoder_window_backward(dec, state, *cot)
+    one = [*grads, dSpeech, dStyle]
+    grads, dSpeech, dStyle, finish = ops.decoder_window_backward(dec, state, *cot, split=True)
+    finish()
+    two = [*grads, dSpeech, dStyle]
+    torch.cuda.synchronize()
+    assert float(one[0].abs().max()) > 0 and float(one[-1].abs().max()) > 0
+    bad = [n for n, a, b in zip(ops._DEC_GRAD_NAMES + ["dSpeech", "dStyle"], one, two) if not torch.equal(a, b)]
+    assert not bad, bad
 
 
 # ---------------------------------------------------------------------------------------------- loudness normalisation + int16 decode (SURVEY 8f row 4)

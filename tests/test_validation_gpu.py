@@ -93,6 +93,26 @@ def test_evaluate_vs_oracle_loss(dev, decoder_engine, engine, H, style):
         assert terms[18] == 0.0
 
 
+@pytest.mark.parametrize("lanes", ["1", "0"])
+@pytest.mark.parametrize("engine,H", [("fp32", 64), ("tc", 384)])
+def test_evaluate_terms_equal_eval_mode_training_forward(dev, decoder_engine, monkeypatch, engine, H, lanes):
+    """evaluate() and forward_backward(train_mode=False) run the same forward: bitwise-equal loss terms (KL term included), with the
+    concurrent lanes on and off.  evaluate() runs first, on a fresh TrainStep."""
+    decoder_engine(engine)
+    monkeypatch.setenv("ZEGGS_LANES", lanes)
+    step, _ = _make_step(dev, H, "example")
+    assert step.lanes == (lanes == "1")
+    step.iteration = 7000
+    batch = _batch(dev, 4, 16, 24, 33)
+    eps = torch.from_numpy(np.random.RandomState(3).randn(4, 64).astype(np.float32)).to(dev)
+    terms = step.evaluate(batch, eps=eps)
+    step.optimizer.zero_grad()
+    step.forward_backward(batch, eps=eps, train_mode=False)
+    torch.cuda.synchronize()
+    assert terms[18] > 0
+    assert torch.equal(terms, step.terms)
+
+
 def _snapshot(step):
     o, dev = step.optimizer, step.dev
     return dict(grad=o.flat_grad.clone(), param=o.flat_param.clone(), m=o.exp_avg.clone(), v=o.exp_avg_sq.clone(),

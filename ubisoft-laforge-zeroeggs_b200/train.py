@@ -3,6 +3,7 @@ main.py:64-71); `TrainStep` is the step body (train.py:196-432) with every stage
 speech encoder, style encoder (attn or gru, VAE on or off), persistent decoder window (fwd + BPTT), fused FK/L1 loss, fused RAdam,
 and -- when torch.distributed is initialised -- ONE NCCL all-reduce of the flat gradient per step.
 """
+import contextlib
 import datetime
 import json
 import math
@@ -89,12 +90,10 @@ class TrainStep:
         # concurrent lanes: SpeechEncoder next to StyleEncoder in the forward; in the backward both encoders next to the decoder's
         # weight-gradient GEMMs (the many small, latency-bound encoder kernels fill the tail waves of the large GEMMs).  Each lane
         # has its own stream and its own GEMM scratch (ops.lane); fork/join by events, so the pattern captures into the graph as
-        # parallel branches.
-        import os
+        # parallel branches.  The side lanes carry the short latency-bound kernels: high priority, so their CTAs are placed ahead
+        # of the queued GEMM tiles.
         self.lanes = self.dev.type == "cuda" and os.environ.get("ZEGGS_LANES", "1") == "1"
-        # the side lanes carry the short latency-bound kernels: high priority, so their CTAs are placed ahead of the queued GEMM tiles
-        prio = -1 if os.environ.get("ZEGGS_LANE_PRIORITY", "1") == "1" else 0
-        self._lane_streams = [torch.cuda.Stream(self.dev, priority=prio), torch.cuda.Stream(self.dev, priority=prio)] if self.lanes else None
+        self._lane_streams = [torch.cuda.Stream(self.dev, priority=-1) for _ in range(2)] if self.lanes else None
 
     def forward_backward(self, batch, eps=None, masks=None, train_mode=True):
         """batch: dict of DEVICE tensors: audio[B,T,81], the 8 pose tensors [B,T,...], gaze_pos[B,T,3], style (example
@@ -108,77 +107,88 @@ class TrainStep:
                 return self._forward_backward(batch, eps, masks, train_mode)
         return self._forward_backward(batch, eps, masks, train_mode)
 
-    def _forward_backward(self, batch, eps, masks, train_mode):
-        """Explicit forward + backward through the C ABI (no autograd engine on the step): every kernel writes its parameter
-        gradients straight into the optimizer's flat gradient buffer (the views RAdam installed as p.grad)."""
+    @contextlib.contextmanager
+    def _lane(self, i, name, after=None):
+        """With lanes on: the block's calls go to side stream i, in lane `name` (its own GEMM scratch, ops.lane), behind the event
+        `after` (_mark), else behind everything issued so far on the current stream.  With lanes off: the block runs in place."""
+        if not self.lanes:
+            yield
+            return
+        s = self._lane_streams[i]
+        s.wait_event(after if after is not None else torch.cuda.current_stream(self.dev).record_event())
+        with torch.cuda.stream(s), ops.lane(name):
+            yield
+
+    def _mark(self, i=None):
+        """With lanes on: an event after the work issued so far on side stream i, or on the current stream (i=None).  None with
+        lanes off."""
+        if not self.lanes:
+            return None
+        return (torch.cuda.current_stream(self.dev) if i is None else self._lane_streams[i]).record_event()
+
+    def _join(self, *marks):
+        """The current stream waits for each mark (_mark); a None mark is nothing to wait for."""
+        cur = torch.cuda.current_stream(self.dev)
+        for ev in marks:
+            if ev is not None:
+                cur.wait_event(ev)
+
+    def _forward(self, batch, eps, masks, save):
+        """normalise -> SpeechEncoder (lane 0) | the StyleEncoder's draws, then the decoder's weight packs (lane 1) -> StyleEncoder ->
+        decoder window, in the networks' current train / eval mode.  save: keep the activations and build the BPTT weight images for
+        the backward.  -> (the loss's inputs: prediction Y, root_pos, root_rot and ground truth packed pose, root_pos, root_rot,
+        gaze_pos; mu; logvar; the states of the backward), mu = logvar = None without the VAE."""
         se, dec, st = self.se, self.dec, self.st
-        se.train(train_mode); dec.train(train_mode)
-        gv = lambda m: [p.grad for p in m._weights()]
+        masks = masks or {}
+        stats = (self.in_mean, self.in_std, self.out_mean, self.out_std)
         xa = ops.normalize_rows(batch["audio"], self.audio_mean, self.audio_std)
-        cur = torch.cuda.current_stream(self.dev) if self.lanes else None
-        s1, s2 = self._lane_streams if self.lanes else (None, None)
-        prep = None
-        if self.lanes:
-            s1.wait_stream(cur)
-            with torch.cuda.stream(s1), ops.lane("speech"):
-                speech, se_state = ops.speech_encoder_fwd(se, xa, ops.speech_encoder_masks(se, xa, None if masks is None else masks.get("speech")))
-            # second lane: the StyleEncoder's dropout multipliers / VAE noise first (off the main stream's critical chain; same host order
-            # of the seeded draws as without lanes), then the weight-only preparation of the decoder (bf16 weight images, folded layer-2
-            # matrix, BPTT images)
-            s2.wait_stream(cur)
-            with torch.cuda.stream(s2), ops.lane("style"):
-                if st is not None:
-                    st.train(train_mode)
-                    pre_style = ops.style_encoder_prepare(st, batch["style"], eps, None if masks is None else masks.get("style"))
-                    ev_style = torch.cuda.Event()
-                    ev_style.record(s2)
-                prep = ops.decoder_prepack(dec, xa.shape[0], xa.shape[1], self.dev, (self.in_mean, self.in_std, self.out_mean, self.out_std), self.dt)
-        else:
-            speech, se_state = ops.speech_encoder_fwd(se, xa, ops.speech_encoder_masks(se, xa, None if masks is None else masks.get("speech")))
+        with self._lane(0, "speech"):
+            speech, se_state = ops.speech_encoder_fwd(se, xa, ops.speech_encoder_masks(se, xa, masks.get("speech")))
+        # the StyleEncoder's dropout multipliers / VAE noise first (off the main stream's critical chain; seeded draws after the speech
+        # encoder's), then the weight-only preparation of the decoder (bf16 weight images, folded layer-2 matrix, BPTT images)
+        with self._lane(1, "style"):
+            if st is not None:
+                eps, smasks = ops.style_encoder_prepare(st, batch["style"], eps, masks.get("style"))
+                drawn = self._mark(1)
+            ops.decoder_prepack(dec, xa.shape[0], xa.shape[1], self.dev, stats, self.dt, backward=save)
         mu = logvar = st_state = None
         if st is not None:
-            st.train(train_mode)
             xs = ops.normalize_rows(batch["style"], self.in_mean, self.in_std)
-            if self.lanes:
-                eps_, smasks = pre_style
-                cur.wait_event(ev_style)
-            else:
-                eps_, smasks = ops.style_encoder_prepare(st, xs, eps, None if masks is None else masks.get("style"))
-            (z, mu, logvar), st_state = ops.style_encoder_fwd(st, xs, eps_, smasks, 1.0)
+            self._join(drawn)
+            (z, mu, logvar), st_state = ops.style_encoder_fwd(st, xs, eps, smasks, 1.0)
         else:
             z = batch["style"]
-        if self.lanes:
-            cur.wait_stream(s1)
-            cur.wait_stream(s2)
+        self._join(self._mark(0), self._mark(1))
         T = speech.shape[1]
         W = [batch[k] for k in POSE_KEYS]
         WY = pack_pose(*W[2:])                                   # ground-truth window, packed once
         Y, rp, rq, dstate = ops.decoder_window_forward(dec, W[0][:, 0], W[1][:, 0], WY[:, 0], batch["gaze_pos"], speech,
-                                                       z.unsqueeze(1).expand(-1, T, -1),
-                                                       (self.in_mean, self.in_std, self.out_mean, self.out_std), self.dt, save=True)
-        loss, (dY, dRp, dRq, dmu, dlv) = ops.loss_fwd_bwd(Y, rp, rq, WY, W[0], W[1], batch["gaze_pos"], self.parents, self.dt, mu, logvar,
+                                                       z.unsqueeze(1).expand(-1, T, -1), stats, self.dt, save=save)
+        return (Y, rp, rq, WY, W[0], W[1], batch["gaze_pos"]), mu, logvar, (dstate, se_state, st_state)
+
+    def _forward_backward(self, batch, eps, masks, train_mode):
+        """Explicit forward + backward through the C ABI (no autograd engine on the step): every kernel writes its parameter
+        gradients straight into the optimizer's flat gradient buffer (the views RAdam installed as p.grad)."""
+        se, dec, st = self.se, self.dec, self.st
+        for m in (se, dec, st):
+            if m is not None:
+                m.train(train_mode)
+        loss_in, mu, logvar, (dstate, se_state, st_state) = self._forward(batch, eps, masks, save=True)
+        loss, (dY, dRp, dRq, dmu, dlv) = ops.loss_fwd_bwd(*loss_in, self.parents, self.dt, mu, logvar,
                                                           kl_weight(self.iteration) if mu is not None else 0.0, self.terms,
                                                           self.klw if mu is not None else None)
-        if not self.lanes:
-            _, dSpeech, dStyle = ops.decoder_window_backward(dec, dstate, dY, dRp, dRq, grads_out=gv(dec))
-            ops.speech_encoder_bwd(se_state, dSpeech, grads_out=gv(se))
-            if st is not None:
-                ops.style_encoder_bwd(st_state, dStyle.sum(dim=1), dmu, dlv, grads_out=gv(st))     # z was broadcast over the window
-            return loss
-        # phase 1 (recurrence + conditioning gradients) -> fork: encoders' backward on their lanes, phase 2 (weight gradients) here -> join
+        gv = lambda m: [p.grad for p in m._weights()]
+        # phase 1 (recurrence + conditioning gradients), phase 2 (weight gradients); the encoders' backward passes need only phase 1:
+        # with lanes on they run beside phase 2, with lanes off after it -> join
         _, dSpeech, dStyle, finish = ops.decoder_window_backward(dec, dstate, dY, dRp, dRq, grads_out=gv(dec), split=True)
-        s1.wait_stream(cur)
-        with torch.cuda.stream(s1), ops.lane("speech"):
+        phase1 = self._mark()
+        finish()
+        with self._lane(0, "speech", after=phase1):
             ops.speech_encoder_bwd(se_state, dSpeech, grads_out=gv(se))
         if st is not None:
-            s2.wait_stream(cur)
-            with torch.cuda.stream(s2), ops.lane("style"):
+            with self._lane(1, "style", after=phase1):
                 ops.style_encoder_bwd(st_state, dStyle.sum(dim=1), dmu, dlv, grads_out=gv(st))     # z was broadcast over the window
-        keep = finish()
-        cur.wait_stream(s1)
-        if st is not None:
-            cur.wait_stream(s2)
-        del keep
+        self._join(self._mark(0), self._mark(1) if st is not None else None)
         return loss
 
     @torch.no_grad()
@@ -188,30 +198,15 @@ class TrainStep:
         The VAE noise is `eps` if given, else drawn from a generator seeded with (eval_seed, index) -- so the same weights and batch
         give bitwise-identical terms on every call.  Leaves the flat gradient, the optimizer state, `iteration`, `terms`, the
         dropout DeviceSeed, torch's / numpy's / Python's global generators and the captured training graphs alone."""
-        se, dec, st = self.se, self.dec, self.st
-        with eval_mode(se, dec, st):
-            xa = ops.normalize_rows(batch["audio"], self.audio_mean, self.audio_std)
-            speech, _ = ops.speech_encoder_fwd(se, xa, None)
-            mu = logvar = None
-            if st is not None:
-                xs = ops.normalize_rows(batch["style"], self.in_mean, self.in_std)
-                if eps is None and st.use_vae:
-                    g = torch.Generator(device=self.dev)
-                    g.manual_seed(self.eval_seed * 1000003 + int(index))
-                    eps = torch.randn((xs.shape[0], dec.style_encoding_size), generator=g, device=self.dev)
-                eps_, _ = ops.style_encoder_prepare(st, xs, eps, None)
-                (z, mu, logvar), _ = ops.style_encoder_fwd(st, xs, eps_, None, 1.0)
-            else:
-                z = batch["style"]
-            T = speech.shape[1]
-            W = [batch[k] for k in POSE_KEYS]
-            WY = pack_pose(*W[2:])
-            Y, rp, rq, _ = ops.decoder_window_forward(dec, W[0][:, 0], W[1][:, 0], WY[:, 0], batch["gaze_pos"], speech,
-                                                      z.unsqueeze(1).expand(-1, T, -1),
-                                                      (self.in_mean, self.in_std, self.out_mean, self.out_std), self.dt, save=False)
+        if eps is None and self.st is not None and self.st.use_vae:
+            g = torch.Generator(device=self.dev)
+            g.manual_seed(self.eval_seed * 1000003 + int(index))
+            eps = torch.randn((batch["style"].shape[0], self.dec.style_encoding_size), generator=g, device=self.dev)
+        with eval_mode(self.se, self.dec, self.st):
+            loss_in, mu, logvar, _ = self._forward(batch, eps, None, save=False)
             terms = torch.empty(19, dtype=torch.float32, device=self.dev)
-            ops.loss_fwd_bwd(Y, rp, rq, WY, W[0], W[1], batch["gaze_pos"], self.parents, self.dt, mu, logvar,
-                             kl_weight(self.iteration) if mu is not None else 0.0, terms, grad=False)
+            ops.loss_fwd_bwd(*loss_in, self.parents, self.dt, mu, logvar, kl_weight(self.iteration) if mu is not None else 0.0, terms,
+                             grad=False)
         return terms
 
     def _allreduce(self):
