@@ -197,6 +197,34 @@ size_t zeggs_decoder_bwd_tc_workspace_bytes(int H, int S, int Z);
 int zeggs_decoder_pack_weights_bwd_tc(const zeggs_decoder_fwd_args* a, void* packed, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * FiLM-conditioned decoder (rnn_cond "film": RecurrentDecoderFiLM, modules.py:188-227), fp32 SIMT engine only.  Per step
+ *   a = ELU(W0 [pose, speech] + b0) * g[:H] + be[:H];  GRU x2 on [a, pose, speech];  c = ELU(Wm h1 + bm) * g[H:] + be[H:];  y = W3 c + b3
+ * with g = 1 + Wg style + bg, be = Wb style + bb (both [2H] per (b, t)), then devectorise / root integration as the normal decoder.
+ * `dec` carries everything the normal decoder has, with the FiLM shapes: W0 [H, 1134+S], W_ih0 [3H, H+1134+S], W2 / b2 = layer3
+ * [1131, H]; packed = zeggs_decoder_pack_weights_film output; engine must be 0 (there is no tensor-core FiLM recurrence:
+ * ZEGGS_ERR_UNSUPPORTED).  style is [B,T,Z] and feeds the CellStateEncoder (frame 0) and the two predictors (frames >= 1). */
+typedef struct {
+  zeggs_decoder_fwd_args dec;
+  const float *Wm, *bm;          /* recurrent_decoder.layer2 [H, H] */
+  const float *Wg, *bg;          /* recurrent_decoder.gammas_predictor.linear_layer [2H, Z] */
+  const float *Wb, *bb;          /* recurrent_decoder.betas_predictor.linear_layer [2H, Z] */
+} zeggs_decoder_film_fwd_args;
+/* dec.packed_bwd = zeggs_decoder_pack_weights_bwd_film output; dec.dW2 / db2 = layer3; the predictors' gradients below.  All the work
+ * is done in phase 0 or 1; phase 2 returns at once. */
+typedef struct {
+  zeggs_decoder_bwd_args dec;
+  float *dWm, *dbm, *dWg, *dbg, *dWb, *dbb;
+} zeggs_decoder_film_bwd_args;
+size_t zeggs_decoder_packed_film_bytes(int H, int S, int Z);
+int zeggs_decoder_pack_weights_film(const zeggs_decoder_film_fwd_args* a, float* packed, void* stream);
+size_t zeggs_decoder_film_workspace_bytes(int B, int T, int H, int S, int Z, int save_for_backward);
+int zeggs_decoder_film_window_fwd(const zeggs_decoder_film_fwd_args* a, void* stream);
+size_t zeggs_decoder_packed_bwd_film_bytes(int H, int S, int Z);
+int zeggs_decoder_pack_weights_bwd_film(const zeggs_decoder_film_fwd_args* a, float* packed, void* stream);
+size_t zeggs_decoder_film_bwd_workspace_bytes(int B, int T, int H, int S, int Z);
+int zeggs_decoder_film_window_bwd(const zeggs_decoder_film_fwd_args* f, const zeggs_decoder_film_bwd_args* b, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * SpeechEncoder (modules.py:249-272): conv k1 + ELU + drop -> conv k31 (replicate 'same') + ELU + drop -> Linear + ELU.
  * x is the already normalised feature tensor (train.py:232-234).  mask0/mask1 are dropout multipliers
  * (0 or 1/(1-p), p = 0.2) in [B,T,C] layout, NULL in eval mode.  The workspace keeps the activations for _bwd.

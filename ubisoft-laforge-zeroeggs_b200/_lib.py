@@ -67,6 +67,14 @@ class DecoderBwdArgs(C.Structure):
         [("workspace_bytes", C.c_size_t), ("packed_bwd_tc", C.c_void_p), ("workspace_tc", C.c_void_p), ("phase", C.c_int)])
 
 
+class DecoderFilmFwdArgs(C.Structure):
+    _fields_ = [("dec", DecoderFwdArgs)] + [(n, C.c_void_p) for n in ("Wm", "bm", "Wg", "bg", "Wb", "bb")]
+
+
+class DecoderFilmBwdArgs(C.Structure):
+    _fields_ = [("dec", DecoderBwdArgs)] + [(n, C.c_void_p) for n in ("dWm", "dbm", "dWg", "dbg", "dWb", "dbb")]
+
+
 def _struct(name, ints=(), floats=(), ptrs=(), tail=()):
     fields = [(n, C.c_int) for n in ints] + [(n, C.c_float) for n in floats] + [(n, C.c_void_p) for n in ptrs] + list(tail)
     return type(name, (C.Structure,), {"_fields_": fields})
@@ -125,7 +133,8 @@ def struct_mirrors():
             "zeggs_loss_args": LossArgs, "zeggs_pose_post_args": PosePostArgs, "zeggs_gather_args": GatherArgs,
             "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads,
             "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs,
-            "zeggs_resample_args": ResampleArgs}
+            "zeggs_resample_args": ResampleArgs, "zeggs_decoder_film_fwd_args": DecoderFilmFwdArgs,
+            "zeggs_decoder_film_bwd_args": DecoderFilmBwdArgs}
 
 
 SYMBOLS = [
@@ -160,6 +169,14 @@ SYMBOLS = [
     ("zeggs_decoder_packed_bwd_tc_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_decoder_bwd_tc_workspace_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_decoder_pack_weights_bwd_tc", C.c_int, [C.POINTER(DecoderFwdArgs), C.c_void_p, C.c_void_p]),
+    ("zeggs_decoder_packed_film_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    ("zeggs_decoder_pack_weights_film", C.c_int, [C.POINTER(DecoderFilmFwdArgs), C.c_void_p, C.c_void_p]),
+    ("zeggs_decoder_film_workspace_bytes", C.c_size_t, [C.c_int] * 6),
+    ("zeggs_decoder_film_window_fwd", C.c_int, [C.POINTER(DecoderFilmFwdArgs), C.c_void_p]),
+    ("zeggs_decoder_packed_bwd_film_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    ("zeggs_decoder_pack_weights_bwd_film", C.c_int, [C.POINTER(DecoderFilmFwdArgs), C.c_void_p, C.c_void_p]),
+    ("zeggs_decoder_film_bwd_workspace_bytes", C.c_size_t, [C.c_int] * 5),
+    ("zeggs_decoder_film_window_bwd", C.c_int, [C.POINTER(DecoderFilmFwdArgs), C.POINTER(DecoderFilmBwdArgs), C.c_void_p]),
     ("zeggs_speech_enc_workspace_bytes", C.c_size_t, [C.c_int] * 5),
     ("zeggs_speech_enc_fwd", C.c_int, [C.POINTER(SpeechEncArgs), C.c_void_p]),
     ("zeggs_speech_enc_bwd", C.c_int, [C.POINTER(SpeechEncArgs), C.POINTER(SpeechEncGrads), C.c_void_p]),

@@ -57,9 +57,11 @@ __global__ void pack_decoder_bwd_kernel(DecGeom g, BwdGeom bg, const float* __re
   }
 }
 
-template <int U>
+// FILM: the FiLM decoder's BPTT.  B1 splits in two stages: B1a  dc = W3^T (dY_acc*sigma_out) -> d gamma/beta of layer2, dpre2 (DP2);
+// B1b  dh1 = dh1_acc + Wm^T dpre2.  B3 takes the layer-0 modulation: d gamma/beta of layer0, dpre_a = da * gamma * ELU'.
+template <int U, bool FILM>
 __global__ void __launch_bounds__(256, 1)
-decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, BwdWs bw, BwdArgsDev d) {
+decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, BwdWs bw, BwdArgsDev d, FilmDev f) {
   extern __shared__ __align__(16) float smem[];
   constexpr int RT1 = (U < 8 ? 8 : U) / 4;   // B1 tile rows / 4
   constexpr int RT2 = (2 * U) / 4;           // dual tiles
@@ -80,6 +82,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
   const float* PB3a = d.packed + bg.off3a + (size_t)c * 3 * H * 2 * U;
   const float* PB3b = d.packed + bg.off3b + (size_t)c * bg.n4b * 3 * H * 16;
   const float* PB4 = d.packed + bg.off4 + (size_t)c * bg.n4b * H * 16;
+  const float* PBm = d.packed + bg.total + (size_t)c * H * bg.R1;   // FiLM: PBm[c][k][r] = Wm[k][c*U + r]
   const size_t actH = (size_t)nbt * H * 32, act3 = (size_t)nbt * 3 * H * 32, actX = (size_t)nbt * K1P * 32, act4 = (size_t)nbt * 4 * H * 32;
 
   // R(t): finalise dY_acc[t] from dxp (shared `red`-summed values passed through `dxpv`), write DY[t] (scaled by sigma_out).
@@ -173,11 +176,41 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
   if (!grid_sync(gb)) return;
 
   for (int t = T - 1; t >= 1; --t) {
-    // ------------------------------------------------------------ B1
+    if constexpr (FILM) {
+      // ---------------------------------------------------------- B1a (FiLM: layer3, modulation and ELU of layer2)
+      for (int bt = 0; bt < nbt; ++bt) {
+        float acc[RT1][4];
+        const float* x = bw.DY + t * actX + (size_t)bt * K1P * 32;
+        skinny_gemm<RT1, false>(acc, PB1, x, x, K1P / 16, wstage);
+        reduce_store<RT1>(acc, red);
+        __syncthreads();
+        for (int idx = tid; idx < U * 32; idx += 256) {
+          const int u = idx >> 5, b = idx & 31, j = c * U + u, bgl = bt * 32 + b;
+          const float dc = red_sum<4 * RT1>(red, u, b);
+          const float e = f.E2[t * actH + ((size_t)bt * H + j) * 32 + b];
+          float gm = 1.f;
+          if (bgl < a.B) {
+            const size_t row = ((size_t)bgl * T + t) * 4 * H;
+            gm += f.GB[row + H + j];
+            f.DGB[row + H + j] = dc * e;
+            f.DGB[row + 3 * H + j] = dc;
+          }
+          f.DP2[t * actH + ((size_t)bt * H + j) * 32 + b] = dc * gm * (e > 0.f ? 1.f : e + 1.f);
+        }
+        __syncthreads();
+      }
+      if (!grid_sync(gb)) return;
+    }
+    // ------------------------------------------------------------ B1 (FiLM: B1b)
     for (int bt = 0; bt < nbt; ++bt) {
       float acc[RT1][4];
-      const float* x = bw.DY + t * actX + (size_t)bt * K1P * 32;
-      skinny_gemm<RT1, false>(acc, PB1, x, x, K1P / 16, wstage);
+      if constexpr (FILM) {
+        const float* x = f.DP2 + t * actH + (size_t)bt * H * 32;
+        skinny_gemm<RT1, false>(acc, PBm, x, x, H / 16, wstage);
+      } else {
+        const float* x = bw.DY + t * actX + (size_t)bt * K1P * 32;
+        skinny_gemm<RT1, false>(acc, PB1, x, x, K1P / 16, wstage);
+      }
       reduce_store<RT1>(acc, red);
       __syncthreads();
       for (int idx = tid; idx < U * 32; idx += 256) {
@@ -241,9 +274,23 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
         __syncthreads();
         for (int idx = tid; idx < U * 32; idx += 256) {
           const int u = idx >> 5, b = idx & 31, j = c * U + u;
-          float av = w.A[t * actH + ((size_t)bt * H + j) * 32 + b];
-          float da = red_sum<2 * U>(red, u, b);
-          bw.DPA[t * actH + ((size_t)bt * H + j) * 32 + b] = da * (av > 0.f ? 1.f : av + 1.f);   // ELU'(pre) = a+1 for pre<=0
+          if constexpr (FILM) {
+            const float da = red_sum<2 * U>(red, u, b);
+            const int bgl = bt * 32 + b;
+            const float e = f.E0[t * actH + ((size_t)bt * H + j) * 32 + b];
+            float gm = 1.f;
+            if (bgl < a.B) {
+              const size_t row = ((size_t)bgl * T + t) * 4 * H;
+              gm += f.GB[row + j];
+              f.DGB[row + j] = da * e;
+              f.DGB[row + 2 * H + j] = da;
+            }
+            bw.DPA[t * actH + ((size_t)bt * H + j) * 32 + b] = da * gm * (e > 0.f ? 1.f : e + 1.f);
+          } else {
+            float av = w.A[t * actH + ((size_t)bt * H + j) * 32 + b];
+            float da = red_sum<2 * U>(red, u, b);
+            bw.DPA[t * actH + ((size_t)bt * H + j) * 32 + b] = da * (av > 0.f ? 1.f : av + 1.f);   // ELU'(pre) = a+1 for pre<=0
+          }
           bw.DH0[((size_t)bt * H + j) * 32 + b] = red_sum<2 * U>(red, U + u, b) + dhz0[(bt * U + u) * 32 + b];
         }
         __syncthreads();
@@ -451,18 +498,18 @@ extern "C" size_t zeggs_decoder_bwd_workspace_bytes(int B, int T, int H, int S, 
   return make_bws(nullptr, g, T).bytes;
 }
 
-template <int U>
+template <int U, bool FILM>
 static int launch_bwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdGeom& bg, const DecWs& w, const BwdWs& bw,
-                      const BwdArgsDev& d, cudaStream_t stream) {
+                      const BwdArgsDev& d, const FilmDev& f, cudaStream_t stream) {
   size_t smem = (size_t)(8 * 2 * SkinnyCfg<4>::STG + 8 * 16 * 32 + 2 * g.nbt * U * 32 + g.nbt * bg.n4b * 16 * 32 + g.nbt * 9 * 32 + g.nbt * 7 * 32) * sizeof(float);
-  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int dev = 0, nsm = 0, occ = 0;
   ZCHECK_CUDA(cudaGetDevice(&dev));
   ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_bwd_kernel<U>, 256, smem));
+  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_bwd_kernel<U, FILM>, 256, smem));
   ZCHECK_ARG(occ * nsm >= g.G, "decoder bwd: cooperative grid of %d CTAs does not fit", g.G);
-  void* args[] = {(void*)&a, (void*)&g, (void*)&bg, (void*)&w, (void*)&bw, (void*)&d};
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_bwd_kernel<U>, dim3(g.G), dim3(256), args, smem, stream));
+  void* args[] = {(void*)&a, (void*)&g, (void*)&bg, (void*)&w, (void*)&bw, (void*)&d, (void*)&f};
+  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_bwd_kernel<U, FILM>, dim3(g.G), dim3(256), args, smem, stream));
   count_launch();
   return ZEGGS_OK;
 }
@@ -578,13 +625,50 @@ int dcond_scatter(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args&
   return ZEGGS_OK;
 }
 
+// SIMT weight gradients over the k-major fp32 histories (slots t >= 1); l2in: the history of the output layer's input (h1, or the FiLM
+// decoder's modulated layer-2 output).  The conditioning columns are those of `a` (S + Z, or S alone for the FiLM decoder).
+static int wgrad_simt(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w, const BwdWs& bw,
+                      const float* l2in, cudaStream_t stream) {
+  const int H = a.H, nbt = g.nbt, C = a.S + a.Z, A = g.A, nT = a.T - 1;
+  const long long sH = (long long)nbt * H * 32, s3 = (long long)nbt * 3 * H * 32, sX = (long long)nbt * K1P * 32, sC = (long long)nbt * C * 32;
+  int rc;
+  // output layer: dW2 = DY . l2in[t]^T
+  if ((rc = wgrad(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, l2in + sH, sH, (long long)H * 32, H, nT, nbt, b.dW2, H, stream))) return rc;
+  if ((rc = rowsum(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, nT, nbt, b.db2, stream))) return rc;
+  // GRU layer 1
+  if ((rc = wgrad(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih1, H, stream))) return rc;
+  if ((rc = wgrad(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H1, sH, (long long)H * 32, H, nT, nbt, b.dW_hh1, H, stream))) return rc;
+  if ((rc = rowsum(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih1, stream))) return rc;
+  if ((rc = rowsum(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh1, stream))) return rc;
+  // GRU layer 0: input = [a | x_pose | cond]
+  if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.A + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih0, A + H, stream))) return rc;
+  if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW_ih0 + H, A + H, stream))) return rc;
+  if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW_ih0 + H + P_IN, A + H, stream))) return rc;
+  if ((rc = wgrad(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0, sH, (long long)H * 32, H, nT, nbt, b.dW_hh0, H, stream))) return rc;
+  if ((rc = rowsum(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih0, stream))) return rc;
+  if ((rc = rowsum(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh0, stream))) return rc;
+  // layer0
+  if ((rc = wgrad(bw.DPA + sH, sH, (long long)H * 32, H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW0, A, stream))) return rc;
+  if ((rc = wgrad(bw.DPA + sH, sH, (long long)H * 32, H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW0 + P_IN, A, stream))) return rc;
+  if ((rc = rowsum(bw.DPA + sH, sH, (long long)H * 32, H, nT, nbt, b.db0, stream))) return rc;
+  return ZEGGS_OK;
+}
+
+// d cond[t] = W0[:, 1134:]^T dpre_a + W_ih0[:, H+1134:]^T dgi0   (batched over slots t >= 1)
+static int dcond_gemms(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdWs& bw, cudaStream_t stream) {
+  const int H = a.H, nbt = g.nbt, C = a.S + a.Z, A = g.A, nT = a.T - 1;
+  const long long sH = (long long)nbt * H * 32, s3 = (long long)nbt * 3 * H * 32, sC = (long long)nbt * C * 32;
+  int rc = sgemm_batched_launch(1, C, 32, H, a.W0 + P_IN, A, bw.DPA + sH, 32, nullptr, bw.DCOND + sC, 32, 0, 0, nT * nbt, 0, (long long)H * 32, (long long)C * 32, stream); if (rc) return rc;
+  return sgemm_batched_launch(1, C, 32, 3 * H, a.W_ih0 + H + P_IN, A + H, bw.DGI0 + s3, 32, nullptr, bw.DCOND + sC, 32, 0, 1, nT * nbt, 0, (long long)3 * H * 32, (long long)C * 32, stream);
+}
+
 // fp32 engine: the SIMT BPTT recurrence, then the weight gradients, d cond, the CellStateEncoder backward and the dSpeech / dStyle
 // scatter.  It does all of it in phase 1 (or 0) and nothing in phase 2.
 static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
                                    const BwdWs& bw, cudaStream_t stream) {
   ZCHECK_ARG(b.packed_bwd, "decoder bwd: packed_bwd missing");
   if (b.phase == 2) return ZEGGS_OK;
-  const int H = a.H, T = a.T, nbt = g.nbt, C = a.S + a.Z, A = g.A, nT = T - 1;
+  const int T = a.T, nbt = g.nbt;
   int rc;
   ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
   ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
@@ -592,12 +676,12 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
     const BwdGeom bg = make_bgeom(g);
     BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
     ScopedTimer tm("decoder_bwd", stream);
-    rc = g.U == 4 ? launch_bwd<4>(a, g, bg, w, bw, d, stream) : launch_bwd<8>(a, g, bg, w, bw, d, stream);
+    const FilmDev none = {};
+    rc = g.U == 4 ? launch_bwd<4, false>(a, g, bg, w, bw, d, none, stream) : launch_bwd<8, false>(a, g, bg, w, bw, d, none, stream);
     if (rc) return rc;
   }
   ScopedTimer tm("decoder_wgrad", stream);
   if ((rc = cond_kmajor(a, g, bw, stream))) return rc;
-  const long long sH = (long long)nbt * H * 32, s3 = (long long)nbt * 3 * H * 32, sX = (long long)nbt * K1P * 32, sC = (long long)nbt * C * 32;
   // weight gradients: tensor-core GEMMs over split-bf16 copies of the histories when those fit the scratch buffer (a second, lo pass
   // in GEMM mode 1 for ~fp32 accuracy), the SIMT k-major kernels otherwise
   const bool want_lo = gemm_mode() == 1;
@@ -606,31 +690,25 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
     for (int i = 0; i < NHIST; ++i) if ((rc = split_hist(hs, i, stream))) return rc;
     if ((rc = wgrad_gemms(a, b, g, hs, want_lo, hs.end, stream))) return rc;
   } else {
-    // layer2: dW2 = DY . H1[t]^T
-    if ((rc = wgrad(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, w.H1 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW2, H, stream))) return rc;
-    if ((rc = rowsum(bw.DY + sX, sX, (long long)K1P * 32, P_OUT, nT, nbt, b.db2, stream))) return rc;
-    // GRU layer 1
-    if ((rc = wgrad(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0 + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih1, H, stream))) return rc;
-    if ((rc = wgrad(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, w.H1, sH, (long long)H * 32, H, nT, nbt, b.dW_hh1, H, stream))) return rc;
-    if ((rc = rowsum(bw.DGI1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih1, stream))) return rc;
-    if ((rc = rowsum(bw.DGH1 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh1, stream))) return rc;
-    // GRU layer 0: input = [a | x_pose | cond]
-    if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.A + sH, sH, (long long)H * 32, H, nT, nbt, b.dW_ih0, A + H, stream))) return rc;
-    if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW_ih0 + H, A + H, stream))) return rc;
-    if ((rc = wgrad(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW_ih0 + H + P_IN, A + H, stream))) return rc;
-    if ((rc = wgrad(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, w.H0, sH, (long long)H * 32, H, nT, nbt, b.dW_hh0, H, stream))) return rc;
-    if ((rc = rowsum(bw.DGI0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_ih0, stream))) return rc;
-    if ((rc = rowsum(bw.DGH0 + s3, s3, (long long)3 * H * 32, 3 * H, nT, nbt, b.db_hh0, stream))) return rc;
-    // layer0
-    if ((rc = wgrad(bw.DPA + sH, sH, (long long)H * 32, H, w.XP + sX, sX, (long long)K1P * 32, P_IN, nT, nbt, b.dW0, A, stream))) return rc;
-    if ((rc = wgrad(bw.DPA + sH, sH, (long long)H * 32, H, bw.COND + sC, sC, (long long)C * 32, C, nT, nbt, b.dW0 + P_IN, A, stream))) return rc;
-    if ((rc = rowsum(bw.DPA + sH, sH, (long long)H * 32, H, nT, nbt, b.db0, stream))) return rc;
+    if ((rc = wgrad_simt(a, b, g, w, bw, w.H1, stream))) return rc;
   }
-  // d cond[t] = W0[:, 1134:]^T dpre_a + W_ih0[:, H+1134:]^T dgi0   (batched over slots t >= 1)
-  rc = sgemm_batched_launch(1, C, 32, H, a.W0 + P_IN, A, bw.DPA + sH, 32, nullptr, bw.DCOND + sC, 32, 0, 0, nT * nbt, 0, (long long)H * 32, (long long)C * 32, stream); if (rc) return rc;
-  rc = sgemm_batched_launch(1, C, 32, 3 * H, a.W_ih0 + H + P_IN, A + H, bw.DGI0 + s3, 32, nullptr, bw.DCOND + sC, 32, 0, 1, nT * nbt, 0, (long long)3 * H * 32, (long long)C * 32, stream); if (rc) return rc;
+  if ((rc = dcond_gemms(a, g, bw, stream))) return rc;
   if ((rc = cse_backward(a, b, w, bw, stream))) return rc;
   return dcond_scatter(a, b, g, bw, 0, stream);
+}
+
+// a one-frame window outputs the given first pose (modules.py:72-79): no weight and no conditioning input reaches it, so every
+// gradient is zero (the reference's autograd gives the same).  A: input width of layer0.
+static int zero_window_grads(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, size_t A, cudaStream_t stream) {
+  const size_t H = a.H, Kin = P_IN + a.Z;
+  const struct { float* p; size_t n; } zero[] = {
+      {b.dW0, H * A}, {b.db0, H}, {b.dW_ih0, 3 * H * (A + H)}, {b.db_ih0, 3 * H}, {b.dW_hh0, 3 * H * H}, {b.db_hh0, 3 * H},
+      {b.dW_ih1, 3 * H * H}, {b.db_ih1, 3 * H}, {b.dW_hh1, 3 * H * H}, {b.db_hh1, 3 * H}, {b.dW2, (size_t)P_OUT * H}, {b.db2, (size_t)P_OUT},
+      {b.dWc0, H * Kin}, {b.dbc0, H}, {b.dWc1, H * H}, {b.dbc1, H}, {b.dWc2, 2 * H * H}, {b.dbc2, 2 * H},
+      {b.dSpeech, (size_t)a.B * a.S}, {b.dStyle, (size_t)a.B * a.Z}};
+  for (const auto& z : zero)
+    if (z.p) ZCHECK_CUDA(cudaMemsetAsync(z.p, 0, z.n * sizeof(float), stream));
+  return ZEGGS_OK;
 }
 
 extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const zeggs_decoder_bwd_args* bp, void* stream_) {
@@ -641,20 +719,7 @@ extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const 
   cudaStream_t stream = (cudaStream_t)stream_;
   ZCHECK_ARG(a.save_for_backward && a.workspace, "decoder bwd: forward must have run with save_for_backward=1");
   ZCHECK_ARG(a.T >= 1 && b.phase >= 0 && b.phase <= 2, "decoder bwd: bad T=%d / phase=%d", a.T, b.phase);
-  if (a.T == 1) {
-    // a one-frame window outputs the given first pose (modules.py:72-79): no weight and no conditioning input reaches it, so every
-    // gradient is zero (the reference's autograd gives the same)
-    if (b.phase == 2) return ZEGGS_OK;
-    const size_t H = a.H, A = P_IN + a.S + a.Z, Kin = P_IN + a.Z;
-    const struct { float* p; size_t n; } zero[] = {
-        {b.dW0, H * A}, {b.db0, H}, {b.dW_ih0, 3 * H * (A + H)}, {b.db_ih0, 3 * H}, {b.dW_hh0, 3 * H * H}, {b.db_hh0, 3 * H},
-        {b.dW_ih1, 3 * H * H}, {b.db_ih1, 3 * H}, {b.dW_hh1, 3 * H * H}, {b.db_hh1, 3 * H}, {b.dW2, (size_t)P_OUT * H}, {b.db2, (size_t)P_OUT},
-        {b.dWc0, H * Kin}, {b.dbc0, H}, {b.dWc1, H * H}, {b.dbc1, H}, {b.dWc2, 2 * H * H}, {b.dbc2, 2 * H},
-        {b.dSpeech, (size_t)a.B * a.S}, {b.dStyle, (size_t)a.B * a.Z}};
-    for (const auto& z : zero)
-      if (z.p) ZCHECK_CUDA(cudaMemsetAsync(z.p, 0, z.n * sizeof(float), stream));
-    return ZEGGS_OK;
-  }
+  if (a.T == 1) return b.phase == 2 ? ZEGGS_OK : zero_window_grads(a, b, P_IN + a.S + a.Z, stream);
   DecGeom g = make_geom(a.B, a.H, a.S, a.Z);
   DecWs w = make_ws(a.workspace, g, a.T, 1);
   BwdWs bw = make_bws(b.workspace, g, a.T);
@@ -662,6 +727,147 @@ extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const 
   // a tensor-core forward with no BPTT pack (packed_bwd_tc == NULL) takes the fp32 backward
   if (a.engine == 1 && b.packed_bwd_tc) return decoder_window_bwd_tc(a, b, g, w, bw, stream);
   return decoder_window_bwd_fp32(a, b, g, w, bw, stream);
+}
+
+
+// ------------------------------------------------------------------ FiLM decoder (fp32 engine)
+// PBm[c][k][r] = Wm[k][c*U + r] (r < U, zero up to R1), behind the normal decoder's transposed slices
+__global__ void pack_film_bwd_kernel(DecGeom g, int R1, const float* __restrict__ Wm, float* __restrict__ out) {
+  const int H = g.H, U = g.U;
+  const size_t total = (size_t)g.G * H * R1;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int r = i % R1, k = (i / R1) % H, c = i / ((size_t)R1 * H);
+    out[i] = r < U ? Wm[(size_t)k * H + c * U + r] : 0.f;
+  }
+}
+
+// out[c] = sum over rows of x[r][c] (row stride ld)
+__global__ void colsum_ld_kernel(const float* __restrict__ x, int rows, int cols, int ld, float* __restrict__ out) {
+  int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  float s = 0.f;
+  for (int r = 0; r < rows; ++r) s += x[(size_t)r * ld + c];
+  out[c] = s;
+}
+
+// dStyle[b][0][:] += the CellStateEncoder's input gradient of the style columns (frame 0 has no FiLM term)
+__global__ void film_style0_kernel(int B, int T, int Z, const float* __restrict__ cse_din, float* __restrict__ dStyle) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * Z) return;
+  int b = i / Z, z = i % Z;
+  dStyle[(size_t)b * T * Z + z] += cse_din[(size_t)b * (P_IN + Z) + P_IN + z];
+}
+
+static size_t film_bwd_extra_floats(const DecGeom& g) { return (size_t)g.G * g.H * make_bgeom(g).R1; }
+
+extern "C" size_t zeggs_decoder_packed_bwd_film_bytes(int H, int S, int Z) {
+  if (H % 16 != 0 || pick_U(H) <= 0) return 0;
+  DecGeom g = make_film_geom(1, H, S, Z);
+  return (make_bgeom(g).total + film_bwd_extra_floats(g)) * sizeof(float);
+}
+
+extern "C" int zeggs_decoder_pack_weights_bwd_film(const zeggs_decoder_film_fwd_args* f, float* packed, void* stream_) {
+  CtxScope ctx_scope(f ? f->dec.ctx : nullptr);
+  ZCHECK_ARG(f && packed && f->Wm && f->dec.H % 16 == 0 && pick_U(f->dec.H) > 0, "film decoder bwd pack: bad arguments");
+  const zeggs_decoder_fwd_args& a = f->dec;
+  DecGeom g = make_film_geom(a.B, a.H, a.S, a.Z);
+  BwdGeom bg = make_bgeom(g);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  pack_decoder_bwd_kernel<<<592, 256, 0, stream>>>(g, bg, a.W0, a.W_ih0, a.W_hh0, a.W_ih1, a.W_hh1, a.W2, packed);
+  count_launch();
+  pack_film_bwd_kernel<<<264, 256, 0, stream>>>(g, bg.R1, f->Wm, packed + bg.total);
+  count_launch();
+  ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+// backward workspace: the normal decoder's carve-up followed by DGB [B*T][4H] and DP2 [T][nbt][H][32]
+static size_t film_bwd_ws(void* base, const DecGeom& g, int T, FilmDev& f) {
+  size_t off = make_bws(nullptr, g, T).bytes;
+  auto take = [&](size_t nfloats) {
+    float* p = base ? (float*)((char*)base + off) : nullptr;
+    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
+    return p;
+  };
+  f.DGB = take((size_t)g.B * T * 4 * g.H);
+  f.DP2 = take((size_t)T * g.nbt * g.H * 32);
+  return off;
+}
+
+extern "C" size_t zeggs_decoder_film_bwd_workspace_bytes(int B, int T, int H, int S, int Z) {
+  if (H % 16 != 0 || pick_U(H) <= 0 || B < 1 || T < 1) return 0;
+  FilmDev f = {};
+  return film_bwd_ws(nullptr, make_film_geom(B, H, S, Z), T, f);
+}
+
+extern "C" int zeggs_decoder_film_window_bwd(const zeggs_decoder_film_fwd_args* fp, const zeggs_decoder_film_bwd_args* bp, void* stream_) {
+  CtxScope ctx_scope(fp ? fp->dec.ctx : nullptr);
+  ZCHECK_ARG(fp && bp, "film decoder bwd: null args");
+  const zeggs_decoder_fwd_args& a = fp->dec;
+  const zeggs_decoder_bwd_args& b = bp->dec;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  ZCHECK_ARG(a.save_for_backward && a.workspace, "film decoder bwd: forward must have run with save_for_backward=1");
+  ZCHECK_ARG(a.T >= 1 && b.phase >= 0 && b.phase <= 2, "film decoder bwd: bad T=%d / phase=%d", a.T, b.phase);
+  ZCHECK_SUPPORTED(a.engine == 0, "film decoder bwd: only the fp32 engine (engine 0)");
+  ZCHECK_ARG(b.packed_bwd, "film decoder bwd: packed_bwd missing (call zeggs_decoder_pack_weights_bwd_film)");
+  if (b.phase == 2) return ZEGGS_OK;
+  const int H = a.H, T = a.T, Z = a.Z;
+  if (T == 1) {
+    int rc = zero_window_grads(a, b, P_IN + a.S, stream); if (rc) return rc;
+    const struct { float* p; size_t n; } zero[] = {{bp->dWm, (size_t)H * H}, {bp->dbm, (size_t)H}, {bp->dWg, (size_t)2 * H * Z},
+                                                   {bp->dbg, (size_t)2 * H}, {bp->dWb, (size_t)2 * H * Z}, {bp->dbb, (size_t)2 * H}};
+    for (const auto& z : zero)
+      if (z.p) ZCHECK_CUDA(cudaMemsetAsync(z.p, 0, z.n * sizeof(float), stream));
+    return ZEGGS_OK;
+  }
+  DecGeom g = make_film_geom(a.B, H, a.S, Z);
+  DecWs w = make_ws(a.workspace, g, T, 1);
+  size_t fwd_bytes = 0;
+  FilmDev f = make_film_ws(a.workspace, w, g, T, &fwd_bytes);
+  BwdWs bw = make_bws(b.workspace, g, T);
+  const size_t need = film_bwd_ws(b.workspace, g, T, f);
+  ZCHECK_ARG(a.workspace_bytes >= fwd_bytes, "film decoder bwd: forward workspace too small (%zu < %zu)", a.workspace_bytes, fwd_bytes);
+  ZCHECK_ARG(b.workspace && b.workspace_bytes >= need, "film decoder bwd: workspace too small (%zu < %zu)", b.workspace_bytes, need);
+  const int nbt = g.nbt, BT = a.B * T;
+  int rc;
+  ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
+  ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
+  ZCHECK_CUDA(cudaMemsetAsync(f.DGB, 0, (size_t)BT * 4 * H * sizeof(float), stream));
+  {
+    const BwdGeom bg = make_bgeom(g);
+    BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
+    ScopedTimer tm("decoder_bwd", stream);
+    rc = g.U == 4 ? launch_bwd<4, true>(a, g, bg, w, bw, d, f, stream) : launch_bwd<8, true>(a, g, bg, w, bw, d, f, stream);
+    if (rc) return rc;
+  }
+  ScopedTimer tm("decoder_wgrad", stream);
+  // the recurrence's conditioning input is the speech alone: the normal decoder's host steps with no style columns
+  zeggs_decoder_fwd_args as = a;
+  as.Z = 0;
+  if ((rc = cond_kmajor(as, g, bw, stream))) return rc;
+  if ((rc = wgrad_simt(as, b, g, w, bw, f.C2, stream))) return rc;
+  const long long sH = (long long)nbt * H * 32;
+  if ((rc = wgrad(f.DP2 + sH, sH, (long long)H * 32, H, w.H1 + sH, sH, (long long)H * 32, H, T - 1, nbt, bp->dWm, H, stream))) return rc;
+  if ((rc = rowsum(f.DP2 + sH, sH, (long long)H * 32, H, T - 1, nbt, bp->dbm, stream))) return rc;
+  if ((rc = dcond_gemms(as, g, bw, stream))) return rc;
+  if ((rc = cse_backward(a, b, w, bw, stream))) return rc;
+  if ((rc = dcond_scatter(as, b, g, bw, 0, stream))) return rc;
+  // the predictors (modules.py:215-217): dW = dGB^T style, db = column sums, dStyle = dG Wg + dBe Wb (+ the CellStateEncoder's part)
+  rc = gemm_f32_auto(1, 2 * H, Z, BT, f.DGB, 4 * H, a.style, Z, nullptr, bp->dWg, Z, 0, 0, stream); if (rc) return rc;
+  rc = gemm_f32_auto(1, 2 * H, Z, BT, f.DGB + 2 * H, 4 * H, a.style, Z, nullptr, bp->dWb, Z, 0, 0, stream); if (rc) return rc;
+  colsum_ld_kernel<<<ceil_div(2 * H, 256), 256, 0, stream>>>(f.DGB, BT, 2 * H, 4 * H, bp->dbg);
+  count_launch();
+  colsum_ld_kernel<<<ceil_div(2 * H, 256), 256, 0, stream>>>(f.DGB + 2 * H, BT, 2 * H, 4 * H, bp->dbb);
+  count_launch();
+  ZCHECK_LAUNCH();
+  if (b.dStyle) {
+    rc = gemm_f32_auto(2, BT, Z, 2 * H, f.DGB, 4 * H, fp->Wg, Z, nullptr, b.dStyle, Z, 0, 0, stream); if (rc) return rc;
+    rc = gemm_f32_auto(2, BT, Z, 2 * H, f.DGB + 2 * H, 4 * H, fp->Wb, Z, nullptr, b.dStyle, Z, 0, 1, stream); if (rc) return rc;
+    film_style0_kernel<<<ceil_div(a.B * Z, 256), 256, 0, stream>>>(a.B, T, Z, bw.cse_din, b.dStyle);
+    count_launch();
+    ZCHECK_LAUNCH();
+  }
+  return ZEGGS_OK;
 }
 
 }  // namespace zeggs

@@ -144,6 +144,44 @@ inline DecWs make_ws(void* base, const DecGeom& g, int T, int save) {
   return w;
 }
 
+// FiLM decoder (rnn_cond "film"): what the fp32 recurrences read and write beyond the normal decoder's workspace.  The normal
+// decoder's kernels take a zeroed one.  GB / DGB rows are (b*T + t): [g-1 (2H) | be (2H)] and their gradients (rows t = 0 stay 0).
+struct FilmDev {
+  const float* GB;   // [B*T][4H]  predictor outputs: layer-0 half then layer-2 half of gamma - 1, then of beta
+  const float* bm;   // [H]        layer2 bias
+  float *E0, *E2;    // [TS][nbt][H][32]  ELU outputs of layer0 / layer2 before the modulation (save only)
+  float* C2;         // [TS][nbt][H][32]  modulated layer-2 output: the input of layer3
+  float* DGB;        // backward: [B*T][4H]
+  float* DP2;        // backward: [T][nbt][H][32]  d pre-activation of layer2
+};
+
+// rows of the layer-2 FiLM tile (per-CTA units padded to the 8-row minimum of the skinny GEMM)
+__host__ __device__ inline int film_rows(int U) { return U < 8 ? 8 : U; }
+
+// FiLM forward workspace: the normal decoder's carve-up followed by GB, E0, E2, C2; bytes = the whole workspace
+inline FilmDev make_film_ws(void* base, const DecWs& w, const DecGeom& g, int T, size_t* bytes) {
+  FilmDev f = {};
+  size_t off = w.bytes;
+  auto take = [&](size_t nfloats) {
+    float* p = base ? (float*)((char*)base + off) : nullptr;
+    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
+    return p;
+  };
+  f.GB = take((size_t)g.B * T * 4 * g.H);
+  f.E0 = take(w.save ? (size_t)T * g.nbt * g.H * 32 : 64);
+  f.E2 = take(w.save ? (size_t)T * g.nbt * g.H * 32 : 64);
+  f.C2 = take((size_t)w.TS * g.nbt * g.H * 32);
+  *bytes = off;
+  return f;
+}
+
+// the recurrence's geometry of a FiLM decoder: style does not enter layer0 or the GRU, so their input width is 1134 + S
+inline DecGeom make_film_geom(int B, int H, int S, int Z) {
+  DecGeom g = make_geom(B, H, S, Z);
+  g.A = P_IN + S;
+  return g;
+}
+
 const float* decoder_tc_mfold(const zeggs_decoder_fwd_args& a);   // fp32 [4H][H] fold matrix inside packed_tc
 int decoder_fwd_tc_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream);
 

@@ -140,8 +140,9 @@ __global__ void __launch_bounds__(256) cond_precompute_kernel(zeggs_decoder_fwd_
 }
 
 // ------------------------------------------------------------------ the persistent kernel
-template <int U>
-__global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, DecWs w) {
+// FILM: the FiLM decoder's step (modulated layer0, the extra layer2 stage, layer3 as the output layer; see FilmDev)
+template <int U, bool FILM>
+__global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, DecWs w, FilmDev f) {
   extern __shared__ __align__(16) float smem[];
   constexpr int RT1 = U, RT2 = (6 * U) / 4;
   float* stage = smem;                                  // 8 warps x 2 x STG_MAX
@@ -157,6 +158,8 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
   const float* P2 = a.packed + g.off_p2() + (size_t)c * H * 6 * U;
   const float* P3 = a.packed + g.off_p3() + (size_t)c * H * 6 * U;
   const float* P4 = a.packed + g.off_p4() + (size_t)c * g.n4t * H * 16;
+  constexpr int RTM = (U < 8 ? 8 : U) / 4;       // FiLM layer2 tile (film_rows(U) rows)
+  const float* P5 = a.packed + g.packed_floats() + (size_t)c * H * 4 * RTM;
   const size_t actH = (size_t)nbt * H * 32;      // floats per time slot of an [nbt][H][32] buffer
   const size_t actX = (size_t)nbt * K1P * 32;
 
@@ -173,7 +176,15 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
         const int u = idx >> 5, b = idx & 31, j = c * U + u;
         const float* S = w.S01 + (((size_t)t * nbt + bt) * 4 * H) * 32;
         float pre = red_sum<4 * U>(red, u, b) + S[(size_t)j * 32 + b];
-        w.A[ts * actH + ((size_t)bt * H + j) * 32 + b] = elu_f(pre);
+        if constexpr (FILM) {
+          const int bgl = bt * 32 + b;
+          const float* gb = f.GB + ((size_t)bgl * T + t) * 4 * H;
+          const float e = elu_f(pre);
+          w.A[ts * actH + ((size_t)bt * H + j) * 32 + b] = bgl < a.B ? e * (1.f + gb[j]) + gb[2 * H + j] : e;   // modules.py:219-220
+          if (w.save) f.E0[ts * actH + ((size_t)bt * H + j) * 32 + b] = e;
+        } else {
+          w.A[ts * actH + ((size_t)bt * H + j) * 32 + b] = elu_f(pre);
+        }
 #pragma unroll
         for (int gi = 0; gi < 3; ++gi)
           gi0p[((bt * 3 + gi) * U + u) * 32 + b] = red_sum<4 * U>(red, (1 + gi) * U + u, b) + S[(size_t)(H + gi * H + j) * 32 + b];
@@ -241,9 +252,28 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
       __syncthreads();
     }
     if (!grid_sync(gb)) return;
-    // ------------------------------------------------------------ stage 4 (layer2 + pose integration)
+    if constexpr (FILM) {
+      // ---------------------------------------------------------- stage 3b (FiLM layer2: c = ELU(Wm h1 + bm) * g[H:] + be[H:])
+      for (int bt = 0; bt < nbt; ++bt) {
+        float acc[RTM][4];
+        const float* x = w.H1 + ts * actH + (size_t)bt * H * 32;
+        skinny_gemm<RTM, false>(acc, P5, x, x, H / 16, wstage);
+        reduce_store<RTM>(acc, red);
+        __syncthreads();
+        for (int idx = tid; idx < U * 32; idx += 256) {
+          const int u = idx >> 5, b = idx & 31, j = c * U + u, bgl = bt * 32 + b;
+          const float e = elu_f(red_sum<4 * RTM>(red, u, b) + f.bm[j]);
+          const float* gbr = f.GB + ((size_t)bgl * T + t) * 4 * H;
+          f.C2[ts * actH + ((size_t)bt * H + j) * 32 + b] = bgl < a.B ? e * (1.f + gbr[H + j]) + gbr[3 * H + j] : e;   // modules.py:224-225
+          if (w.save) f.E2[ts * actH + ((size_t)bt * H + j) * 32 + b] = e;
+        }
+        __syncthreads();
+      }
+      if (!grid_sync(gb)) return;
+    }
+    // ------------------------------------------------------------ stage 4 (layer2 -- FiLM: layer3 -- + pose integration)
     for (int bt = 0; bt < nbt; ++bt) {
-      const float* x = w.H1 + ts * actH + (size_t)bt * H * 32;
+      const float* x = (FILM ? f.C2 : w.H1) + ts * actH + (size_t)bt * H * 32;
       float* xpn = w.XP + tn * actX + (size_t)bt * K1P * 32;
       for (int tile = 0; tile < g.n4t; ++tile) {
         float acc[4][4];
@@ -326,18 +356,18 @@ extern "C" size_t zeggs_decoder_workspace_bytes(int B, int T, int H, int S, int 
   return make_ws(nullptr, g, T, save).bytes;
 }
 
-template <int U>
-static int launch_fwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
+template <int U, bool FILM>
+static int launch_fwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, const FilmDev& f, cudaStream_t stream) {
   constexpr int RT2 = (6 * U) / 4;
   size_t smem = (size_t)(8 * 2 * SkinnyCfg<RT2>::STG + 8 * 6 * U * 32 + g.nbt * 3 * U * 32 + 6 * 32) * sizeof(float);
-  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_fwd_kernel<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_fwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int dev = 0, nsm = 0, occ = 0;
   ZCHECK_CUDA(cudaGetDevice(&dev));
   ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_fwd_kernel<U>, 256, smem));
+  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_fwd_kernel<U, FILM>, 256, smem));
   ZCHECK_ARG(occ * nsm >= g.G, "decoder: cooperative grid of %d CTAs does not fit (%d SMs x %d)", g.G, nsm, occ);
-  void* args[] = {(void*)&a, (void*)&g, (void*)&w};
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_fwd_kernel<U>, dim3(g.G), dim3(256), args, smem, stream));
+  void* args[] = {(void*)&a, (void*)&g, (void*)&w, (void*)&f};
+  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_fwd_kernel<U, FILM>, dim3(g.G), dim3(256), args, smem, stream));
   count_launch();
   return ZEGGS_OK;
 }
@@ -351,19 +381,13 @@ static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& 
   count_launch();
   ZCHECK_LAUNCH();
   ScopedTimer tm("decoder_fwd", stream);
-  return g.U == 4 ? launch_fwd<4>(a, g, w, stream) : launch_fwd<8>(a, g, w, stream);
+  const FilmDev none = {};
+  return g.U == 4 ? launch_fwd<4, false>(a, g, w, none, stream) : launch_fwd<8, false>(a, g, w, none, stream);
 }
 
-extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* stream_) {
-  int rc = check_fwd_args(ap); if (rc) return rc;
-  const zeggs_decoder_fwd_args& a = *ap;
-  CtxScope ctx_scope(a.ctx);
-  cudaStream_t stream = (cudaStream_t)stream_;
-  DecGeom g = make_geom(a.B, a.H, a.S, a.Z);
-  DecWs w = make_ws(a.workspace, g, a.T, a.save_for_backward);
-  ZCHECK_ARG(a.workspace != nullptr && a.workspace_bytes >= w.bytes, "decoder: workspace too small (%zu < %zu)", a.workspace_bytes, w.bytes);
-  ZCHECK_ARG(a.engine == 1 || a.packed != nullptr, "decoder: packed weights missing (call zeggs_decoder_pack_weights)");
-  ZCHECK_SUPPORTED(a.engine != 1 || tc_hidden_ok(a.H), "decoder tc engine: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", a.H);
+// frame 0 and the initial GRU state (modules.py:72-98), shared by both decoders
+static int decoder_fwd_prologue(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
+  int rc;
   // zero: barrier words, the x_pose slots (k padding rows / batch padding columns) and the h slot 0
   ZCHECK_CUDA(cudaMemsetAsync(w.bar, 0, 256, stream));
   ZCHECK_CUDA(cudaMemsetAsync(w.XP, 0, (size_t)w.TS * g.nbt * K1P * 32 * sizeof(float), stream));
@@ -379,8 +403,101 @@ extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* 
   cse_scatter_kernel<<<ceil_div(a.B * 2 * a.H, 256), 256, 0, stream>>>(a.B, a.H, w.cse_out, w.H0, w.H1);
   count_launch();
   ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* stream_) {
+  int rc = check_fwd_args(ap); if (rc) return rc;
+  const zeggs_decoder_fwd_args& a = *ap;
+  CtxScope ctx_scope(a.ctx);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  DecGeom g = make_geom(a.B, a.H, a.S, a.Z);
+  DecWs w = make_ws(a.workspace, g, a.T, a.save_for_backward);
+  ZCHECK_ARG(a.workspace != nullptr && a.workspace_bytes >= w.bytes, "decoder: workspace too small (%zu < %zu)", a.workspace_bytes, w.bytes);
+  ZCHECK_ARG(a.engine == 1 || a.packed != nullptr, "decoder: packed weights missing (call zeggs_decoder_pack_weights)");
+  ZCHECK_SUPPORTED(a.engine != 1 || tc_hidden_ok(a.H), "decoder tc engine: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", a.H);
+  if ((rc = decoder_fwd_prologue(a, g, w, stream))) return rc;
   if (a.T == 1) return ZEGGS_OK;
   return a.engine == 1 ? decoder_fwd_tc_run(a, g, w, stream) : decoder_fwd_fp32_run(a, g, w, stream);
+}
+
+// ------------------------------------------------------------------ FiLM decoder (fp32 engine)
+// P5[c][k][r] = Wm[c*U + r][k] (r < U; rows up to film_rows(U) are zero), behind the normal decoder's slices
+__global__ void pack_film_kernel(DecGeom g, const float* __restrict__ Wm, float* __restrict__ out) {
+  const int H = g.H, U = g.U, R = film_rows(g.U);
+  const size_t total = (size_t)g.G * H * R;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int r = i % R, k = (i / R) % H, c = i / ((size_t)R * H);
+    out[i] = r < U ? Wm[(size_t)(c * U + r) * H + k] : 0.f;
+  }
+}
+
+static int check_film_args(const zeggs_decoder_film_fwd_args* f) {
+  ZCHECK_ARG(f != nullptr, "film decoder: null args");
+  int rc = check_fwd_args(&f->dec); if (rc) return rc;
+  ZCHECK_SUPPORTED(f->dec.engine == 0, "film decoder: only the fp32 engine (engine 0) runs the FiLM recurrence: its layer2 carries an ELU "
+                                       "and a modulation, so the tensor-core engine's layer-2 fold does not apply");
+  ZCHECK_ARG(f->Wm && f->bm && f->Wg && f->bg && f->Wb && f->bb, "film decoder: layer2 / predictor weights missing");
+  return ZEGGS_OK;
+}
+
+static size_t film_packed_floats(const DecGeom& g) { return g.packed_floats() + (size_t)g.G * g.H * film_rows(g.U); }
+
+extern "C" size_t zeggs_decoder_packed_film_bytes(int H, int S, int Z) {
+  if (H % 16 != 0 || pick_U(H) <= 0) return 0;
+  return film_packed_floats(make_film_geom(1, H, S, Z)) * sizeof(float);
+}
+
+extern "C" int zeggs_decoder_pack_weights_film(const zeggs_decoder_film_fwd_args* f, float* packed, void* stream_) {
+  CtxScope ctx_scope(f ? f->dec.ctx : nullptr);
+  int rc = check_film_args(f); if (rc) return rc;
+  const zeggs_decoder_fwd_args& a = f->dec;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  DecGeom g = make_film_geom(a.B, a.H, a.S, a.Z);
+  pack_decoder_kernel<<<592, 256, 0, stream>>>(g, a.W0, a.W_ih0, a.W_hh0, a.W_ih1, a.W_hh1, a.W2, packed);
+  count_launch();
+  pack_film_kernel<<<264, 256, 0, stream>>>(g, f->Wm, packed + g.packed_floats());
+  count_launch();
+  ZCHECK_LAUNCH();
+  return ZEGGS_OK;
+}
+
+extern "C" size_t zeggs_decoder_film_workspace_bytes(int B, int T, int H, int S, int Z, int save) {
+  if (H % 16 != 0 || pick_U(H) <= 0 || B < 1 || T < 1) return 0;
+  DecGeom g = make_film_geom(B, H, S, Z);
+  size_t bytes = 0;
+  make_film_ws(nullptr, make_ws(nullptr, g, T, save), g, T, &bytes);
+  return bytes;
+}
+
+extern "C" int zeggs_decoder_film_window_fwd(const zeggs_decoder_film_fwd_args* fp, void* stream_) {
+  int rc = check_film_args(fp); if (rc) return rc;
+  const zeggs_decoder_fwd_args& a = fp->dec;
+  CtxScope ctx_scope(a.ctx);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  DecGeom g = make_film_geom(a.B, a.H, a.S, a.Z);
+  DecWs w = make_ws(a.workspace, g, a.T, a.save_for_backward);
+  size_t bytes = 0;
+  FilmDev f = make_film_ws(a.workspace, w, g, a.T, &bytes);
+  f.bm = fp->bm;
+  ZCHECK_ARG(a.workspace != nullptr && a.workspace_bytes >= bytes, "film decoder: workspace too small (%zu < %zu)", a.workspace_bytes, bytes);
+  ZCHECK_ARG(a.packed != nullptr, "film decoder: packed weights missing (call zeggs_decoder_pack_weights_film)");
+  if ((rc = decoder_fwd_prologue(a, g, w, stream))) return rc;
+  if (a.T == 1) return ZEGGS_OK;
+  // gamma - 1 and beta of every (b, t) as two GEMMs through the front end (modules.py:215-217)
+  float* GB = const_cast<float*>(f.GB);
+  rc = gemm_f32_auto(0, a.B * a.T, 2 * a.H, a.Z, a.style, a.Z, fp->Wg, a.Z, fp->bg, GB, 4 * a.H, 0, 0, stream); if (rc) return rc;
+  rc = gemm_f32_auto(0, a.B * a.T, 2 * a.H, a.Z, a.style, a.Z, fp->Wb, a.Z, fp->bb, GB + 2 * a.H, 4 * a.H, 0, 0, stream); if (rc) return rc;
+  // the speech columns of layer0 / GRU0 hoisted out of the recurrence: the normal decoder's pre-pass with no style columns
+  zeggs_decoder_fwd_args as = a;
+  as.Z = 0;
+  const size_t sm = (size_t)(a.S * 33 + 64 * (a.S + 1)) * sizeof(float);
+  ZCHECK_CUDA(cudaFuncSetAttribute(cond_precompute_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  cond_precompute_kernel<<<dim3(a.T, g.nbt, ceil_div(4 * a.H, 64)), 256, sm, stream>>>(as, g, w.S01);
+  count_launch();
+  ZCHECK_LAUNCH();
+  ScopedTimer tm("decoder_fwd", stream);
+  return g.U == 4 ? launch_fwd<4, true>(a, g, w, f, stream) : launch_fwd<8, true>(a, g, w, f, stream);
 }
 
 }  // namespace zeggs

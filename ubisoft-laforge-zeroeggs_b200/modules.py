@@ -36,6 +36,20 @@ class RecurrentDecoderNormal(nn.Module):
         self.layer2 = nn.Linear(hidden_size, output_size)
 
 
+class RecurrentDecoderFiLM(nn.Module):
+    """Parameter container of modules.py:188-227 (keys gammas_predictor.*, betas_predictor.*, layer0.*, layer1.*, layer2.*, layer3.*)."""
+
+    def __init__(self, pose_input_size, speech_size, style_size, output_size, hidden_size, num_rnn_layers):
+        super().__init__()
+        self.hidden_size = hidden_size
+        self.gammas_predictor = LinearNorm(style_size, hidden_size * 2, w_init_gain="linear")
+        self.betas_predictor = LinearNorm(style_size, hidden_size * 2, w_init_gain="linear")
+        self.layer0 = nn.Linear(pose_input_size + speech_size, hidden_size)
+        self.layer1 = nn.GRU(pose_input_size + speech_size + hidden_size, hidden_size, num_rnn_layers, batch_first=True, dropout=0.0)
+        self.layer2 = nn.Linear(hidden_size, hidden_size)
+        self.layer3 = nn.Linear(hidden_size, output_size)
+
+
 class CellStateEncoder(nn.Module):
     """Parameter container of modules.py:230-243."""
 
@@ -48,23 +62,30 @@ class CellStateEncoder(nn.Module):
 
 
 class Decoder(nn.Module):
-    """modules.py:11-162.  forward() = one launch sequence of zeggs_decoder_window_fwd (+ _bwd under autograd)."""
+    """modules.py:11-162.  forward() = one launch sequence of zeggs_decoder_window_fwd (+ _bwd under autograd); with
+    rnn_cond="film", of zeggs_decoder_film_window_fwd (+ _bwd)."""
 
     def __init__(self, pose_input_size, pose_output_size, speech_encoding_size, style_encoding_size,
                  hidden_size, num_rnn_layers, rnn_cond="normal"):
         super().__init__()
-        if rnn_cond != "normal":
-            raise _lib.ZeggsError("only rnn_cond='normal' is on the accelerated path (the shipped configs)")
+        if rnn_cond not in ("normal", "film"):
+            raise _lib.ZeggsError(f"unknown rnn_cond {rnn_cond!r} (modules.py:24-41 knows 'normal' and 'film')")
         if num_rnn_layers != 2:
             raise _lib.ZeggsError("num_rnn_layers must be 2 (train.py:124-131 hard-codes it)")
         if pose_input_size != P_IN or pose_output_size != P_OUT:
             raise _lib.ZeggsError("pose layout must be the 75-joint 1134/1131 layout (modules.py:699-736)")
-        self.recurrent_decoder = RecurrentDecoderNormal(
+        cls = RecurrentDecoderFiLM if rnn_cond == "film" else RecurrentDecoderNormal
+        self.recurrent_decoder = cls(
             pose_input_size, speech_encoding_size, style_encoding_size, pose_output_size, hidden_size, num_rnn_layers)
         self.cell_state_encoder = CellStateEncoder(pose_input_size + style_encoding_size, hidden_size, num_rnn_layers)
 
     # sizes are read off the parameters so that instances un-pickled from the reference's whole-module checkpoints
     # (generate.py:130-138; they carry no extra attributes) work unchanged
+    @property
+    def film(self):
+        """True for rnn_cond="film" (read off the recurrent decoder's class, as whole-module pickles store no option)."""
+        return isinstance(self.recurrent_decoder, RecurrentDecoderFiLM)
+
     @property
     def hidden_size(self):
         return self.recurrent_decoder.layer0.weight.shape[0]
@@ -75,15 +96,23 @@ class Decoder(nn.Module):
 
     @property
     def speech_encoding_size(self):
-        return self.recurrent_decoder.layer0.weight.shape[1] - P_IN - self.style_encoding_size
+        # the FiLM decoder's layer0 sees [pose, speech]; the normal one's [pose, speech, style]
+        return self.recurrent_decoder.layer0.weight.shape[1] - P_IN - (0 if self.film else self.style_encoding_size)
 
     def _weights(self):
+        """Every parameter, in the order of the C ABI's gradient fields: the normal decoder's 18 (for the FiLM decoder the output layer
+        layer3 takes layer2's place), then the FiLM decoder's layer2, gammas_predictor and betas_predictor."""
         r, c = self.recurrent_decoder, self.cell_state_encoder
-        return [r.layer0.weight, r.layer0.bias,
-                r.layer1.weight_ih_l0, r.layer1.bias_ih_l0, r.layer1.weight_hh_l0, r.layer1.bias_hh_l0,
-                r.layer1.weight_ih_l1, r.layer1.bias_ih_l1, r.layer1.weight_hh_l1, r.layer1.bias_hh_l1,
-                r.layer2.weight, r.layer2.bias,
-                c.layer0.weight, c.layer0.bias, c.layer1.weight, c.layer1.bias, c.layer2.weight, c.layer2.bias]
+        out = r.layer3 if self.film else r.layer2
+        w = [r.layer0.weight, r.layer0.bias,
+             r.layer1.weight_ih_l0, r.layer1.bias_ih_l0, r.layer1.weight_hh_l0, r.layer1.bias_hh_l0,
+             r.layer1.weight_ih_l1, r.layer1.bias_ih_l1, r.layer1.weight_hh_l1, r.layer1.bias_hh_l1,
+             out.weight, out.bias,
+             c.layer0.weight, c.layer0.bias, c.layer1.weight, c.layer1.bias, c.layer2.weight, c.layer2.bias]
+        if self.film:
+            g, b = r.gammas_predictor.linear_layer, r.betas_predictor.linear_layer
+            w += [r.layer2.weight, r.layer2.bias, g.weight, g.bias, b.weight, b.bias]
+        return w
 
     def forward(self, Z_root_pos, Z_root_rot, Z_root_vel, Z_root_vrt, Z_lpos, Z_ltxy, Z_lvel, Z_lvrt,
                 Z_gaze_pos, speech_encoding, style_encoding, parents, anim_input_mean, anim_input_std,

@@ -120,9 +120,16 @@ def set_decoder_engine(name):
         c.fast_wgrad = 0 if name == "fp32" else 1
 
 
-def resolve_engine(H, S, Z):
-    """-> True when the tensor-core engine runs this geometry under the current setting."""
+def resolve_engine(H, S, Z, film=False):
+    """-> True when the tensor-core engine runs this geometry under the current setting.  A FiLM decoder always runs on the fp32
+    engine ("auto" picks it); an explicit "tc" raises."""
     if DECODER_ENGINE == "fp32":
+        return False
+    if film:
+        if DECODER_ENGINE == "tc":
+            raise _lib.ZeggsError("decoder engine 'tc' requested for a FiLM decoder (rnn_cond='film'): its layer2 is followed by an ELU "
+                                  "and the FiLM modulation, so the tensor-core engine's fold of layer2 into the next step does not "
+                                  "apply; use 'fp32' or 'auto'")
         return False
     ok = tc_eligible(H, S, Z)
     if DECODER_ENGINE == "tc" and not ok:
@@ -172,16 +179,17 @@ def split_pose(Y, root_pos, root_rot):
 
 
 def _weight_pack(dec, kind, a, dev):
-    """Device buffer of the decoder's weight pack `kind` -- "" (fp32 forward), "_tc", "_bwd" or "_bwd_tc": the output of
+    """Device buffer of the decoder's weight pack `kind` -- "" (fp32 forward), "_tc", "_bwd", "_bwd_tc", "_film" or "_bwd_film": the output of
     zeggs_decoder_pack_weights<kind> -- cached on the module as `_zeggs_packed<kind>` and re-packed whenever any parameter's version
     counter moved or the device changed."""
     l = _lib.lib()
     ver = weights_key(dec._weights())
     cache = dec.__dict__.get("_zeggs_packed" + kind)
     if cache is None or cache[0] != ver or cache[1].device != dev:
-        nbytes = getattr(l, f"zeggs_decoder_packed{kind}_bytes")(a.H, a.S, a.Z)
+        d = a.dec if isinstance(a, _lib.DecoderFilmFwdArgs) else a
+        nbytes = getattr(l, f"zeggs_decoder_packed{kind}_bytes")(d.H, d.S, d.Z)
         if nbytes == 0:
-            raise _lib.ZeggsError(f"decoder hidden size {a.H} unsupported")
+            raise _lib.ZeggsError(f"decoder hidden size {d.H} unsupported")
         packed = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         name = f"zeggs_decoder_pack_weights{kind}"
         _lib.check(getattr(l, name)(a, packed.data_ptr(), _lib.stream_ptr()), name)
@@ -189,9 +197,14 @@ def _weight_pack(dec, kind, a, dev):
     return cache[1]
 
 
+_FILM_NAMES = ["Wm", "bm", "Wg", "bg", "Wb", "bb"]
+
+
 def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
-    """Fill a DecoderFwdArgs; returns (args, keepalive list).  pack_only: stop after the weight packs (decoder_prepack)."""
+    """Fill a DecoderFwdArgs (a DecoderFilmFwdArgs for a FiLM decoder); returns (args, keepalive list, workspace).  pack_only: stop
+    after the weight packs (decoder_prepack)."""
     H, S, Z = dec.hidden_size, dec.speech_encoding_size, dec.style_encoding_size
+    film = dec.film
     l = _lib.lib()
     w = [_f32c(p, dev) for p in dec._weights()]
     names = ["W0", "b0", "W_ih0", "b_ih0", "W_hh0", "b_hh0", "W_ih1", "b_ih1", "W_hh1", "b_hh1", "W2", "b2",
@@ -207,6 +220,20 @@ def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
     for n, t in tensors.items():
         setattr(a, n, _lib.ptr(t))
         keep.append(t)
+    if film:
+        resolve_engine(H, S, Z, film=True)           # raises on an explicit "tc"
+        f = _lib.DecoderFilmFwdArgs(dec=a)
+        for n, t in zip(_FILM_NAMES, w[18:]):
+            setattr(f, n, _lib.ptr(t))
+        f.dec.packed = _weight_pack(dec, "_film", f, dev).data_ptr()
+        keep.append(dec.__dict__["_zeggs_packed_film"][1])
+        if pack_only:
+            return f, keep, None
+        wsb = l.zeggs_decoder_film_workspace_bytes(B, T, H, S, Z, int(save))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if save else WS.get("dec_fwd", wsb, dev)
+        f.dec.workspace, f.dec.workspace_bytes, f.dec.save_for_backward = ws.data_ptr(), wsb, int(save)
+        keep.append(ws)
+        return f, keep, ws
     # each engine packs only its own slices
     use_tc = resolve_engine(H, S, Z)
     if use_tc and B > 32:
@@ -236,7 +263,9 @@ def decoder_prepack(dec, B, T, dev, stats, dt, backward=True):
     (backward=True) the transposed images of the BPTT kernel -- issued on the current stream and lane.  The window calls find the caches
     fresh and skip the work, so a training step can run this next to the encoders' forward instead of in front of the recurrence."""
     a, keep, _ = _decoder_args(dec, B, T, dev, {}, stats, dt, False, pack_only=True)
-    if backward and a.engine == 1:
+    if backward and dec.film:
+        _weight_pack(dec, "_bwd_film", a, dev)
+    elif backward and a.engine == 1:
         _weight_pack(dec, "_bwd_tc", a, dev)
     return keep
 
@@ -257,7 +286,8 @@ def decoder_window_forward(dec, root_pos0, root_rot0, pose0, gaze_pos, speech, s
     rq = torch.empty((B, T, 4), dtype=torch.float32, device=dev)
     tensors.update(Y=Y, root_pos=rp, root_rot=rq)
     a, keep, ws = _decoder_args(dec, B, T, dev, tensors, stats, dt, save)
-    _lib.check(_lib.lib().zeggs_decoder_window_fwd(a, _lib.stream_ptr()), "zeggs_decoder_window_fwd")
+    fn = "zeggs_decoder_film_window_fwd" if dec.film else "zeggs_decoder_window_fwd"
+    _lib.check(getattr(_lib.lib(), fn)(a, _lib.stream_ptr()), fn)
     return Y, rp, rq, (a, keep, ws)
 
 
@@ -283,10 +313,12 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
     calling it issues phase 2 (all remaining parameter gradients) on the then-current stream of the same lane -- the caller may run the
     encoders' backward passes on other streams / lanes in between."""
     l = _lib.lib()
-    a, keep, ws = state
+    fa, keep, ws = state
+    a = fa.dec if dec.film else fa
     dev = ws.device
     B, T, H, S, Z = a.B, a.T, a.H, a.S, a.Z
-    b = _lib.DecoderBwdArgs()
+    fb = _lib.DecoderFilmBwdArgs() if dec.film else None
+    b = fb.dec if dec.film else _lib.DecoderBwdArgs()
     hold = []
     for name, g in (("dY", dY), ("dRootPos", dRp), ("dRootRot", dRq)):
         if g is not None:
@@ -294,7 +326,11 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
             hold.append(g)
             setattr(b, name, g.data_ptr())
     # transposed weight slices for the backward recurrence
-    if a.engine == 1:
+    if dec.film:
+        packed = _weight_pack(dec, "_bwd_film", fa, dev)
+        b.packed_bwd = packed.data_ptr()
+        hold.append(packed)
+    elif a.engine == 1:
         ptc = _weight_pack(dec, "_bwd_tc", a, dev)
         wtc = WS.get("dec_bwd_tc", l.zeggs_decoder_bwd_tc_workspace_bytes(H, S, Z), dev)
         b.packed_bwd_tc, b.workspace_tc = ptc.data_ptr(), wtc.data_ptr()
@@ -306,22 +342,26 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
     grads = _grad_targets(dec._weights(), grads_out)
     for n, g in zip(_DEC_GRAD_NAMES, grads):
         setattr(b, n, g.data_ptr())
+    for n, g in zip(_FILM_NAMES, grads[18:]):
+        setattr(fb, "d" + n, g.data_ptr())
     dSpeech = torch.empty((B, T, S), dtype=torch.float32, device=dev)
     dStyle = torch.empty((B, T, Z), dtype=torch.float32, device=dev)
     b.dSpeech, b.dStyle = dSpeech.data_ptr(), dStyle.data_ptr()
-    wsb = l.zeggs_decoder_bwd_workspace_bytes(B, T, H, S, Z)
+    wsb = (l.zeggs_decoder_film_bwd_workspace_bytes if dec.film else l.zeggs_decoder_bwd_workspace_bytes)(B, T, H, S, Z)
     bws = WS.get("dec_bwd", wsb, dev)
     b.workspace, b.workspace_bytes = bws.data_ptr(), wsb
+    name = "zeggs_decoder_film_window_bwd" if dec.film else "zeggs_decoder_window_bwd"
+    run = (lambda: getattr(l, name)(fa, fb, _lib.stream_ptr())) if dec.film else (lambda: getattr(l, name)(a, b, _lib.stream_ptr()))
     if not split:
-        _lib.check(l.zeggs_decoder_window_bwd(a, b, _lib.stream_ptr()), "zeggs_decoder_window_bwd")
+        _lib.check(run(), name)
         return grads, dSpeech, dStyle
     b.phase = 1
-    _lib.check(l.zeggs_decoder_window_bwd(a, b, _lib.stream_ptr()), "zeggs_decoder_window_bwd (phase 1)")
+    _lib.check(run(), name + " (phase 1)")
 
     def finish():
         b.phase = 2
-        _lib.check(l.zeggs_decoder_window_bwd(a, b, _lib.stream_ptr()), "zeggs_decoder_window_bwd (phase 2)")
-        return hold, bws, grads, state        # everything phase 2 reads stays referenced until it has been issued
+        _lib.check(run(), name + " (phase 2)")
+        return hold, bws, grads, state, fb    # everything phase 2 reads stays referenced until it has been issued
     return grads, dSpeech, dStyle, finish
 
 
@@ -362,7 +402,7 @@ def decoder_window(dec, root_pos0, root_rot0, pose0, gaze_pos, speech, style,
     if speech.device.type != "cuda":
         raise _lib.ZeggsError("zeggs_b200.Decoder runs on CUDA tensors only (no CPU fallback)")
     B = speech.shape[0]
-    if B > 32 and resolve_engine(dec.hidden_size, dec.speech_encoding_size, dec.style_encoding_size):
+    if B > 32 and resolve_engine(dec.hidden_size, dec.speech_encoding_size, dec.style_encoding_size, dec.film):
         # the tensor-core recurrence works on one 32-sample batch tile: independent windows -> run the tiles back to back
         outs = [decoder_window(dec, root_pos0[i:i + 32], root_rot0[i:i + 32], pose0[i:i + 32], gaze_pos[i:i + 32],
                                speech[i:i + 32], style[i:i + 32], in_mean, in_std, out_mean, out_std, dt)
@@ -711,6 +751,8 @@ def decoder_step(dec, pose, speech, style, state):
     style [B,Z], state [2,B,H] -> (y [B,1131] normalised, new state [2,B,H])."""
     if pose.device.type != "cuda":
         raise _lib.ZeggsError("decoder_step runs on CUDA tensors only (no CPU fallback)")
+    if dec.film:
+        raise _lib.ZeggsError("decoder_step covers the normal decoder (RecurrentDecoderNormal); run a FiLM decoder through decoder_window")
     l = _lib.lib()
     dev = pose.device
     w = [_f32c(p, dev) for p in dec._weights()[:12]]

@@ -26,9 +26,12 @@ def _u(rs, shape, bound):
     return rs.uniform(-bound, bound, size=shape).astype(np.float32)
 
 
-def make_params(H=1024, S=64, Z=64, style_hidden=512, style_embed=128, seed=1234, with_style=True, style_type="attn"):
+def make_params(H=1024, S=64, Z=64, style_hidden=512, style_embed=128, seed=1234, with_style=True, style_type="attn",
+                rnn_cond="normal"):
     """Random weights with PyTorch-default-like scales for every tensor on the path.  style_embed is the style encoder's
-    output size (2*Z with the VAE, Z without); style_type 'attn' (StyleEncoderAttn) or 'gru' (StyleEncoderGRU)."""
+    output size (2*Z with the VAE, Z without); style_type 'attn' (StyleEncoderAttn) or 'gru' (StyleEncoderGRU); rnn_cond
+    'normal' (RecurrentDecoderNormal) or 'film' (RecurrentDecoderFiLM: its tensors come from a generator of their own, every other
+    tensor is the one rnn_cond='normal' gives)."""
     rs = np.random.RandomState(seed)
     A = P_IN + S + Z
     P = {}
@@ -100,6 +103,35 @@ def make_params(H=1024, S=64, Z=64, style_hidden=512, style_embed=128, seed=1234
         P[f + "convs.2.conv.bias"] = _u(rs, (E,), 1 / np.sqrt(E * 3))
         P[f + "layer_norm.weight"] = (1 + 0.1 * rs.randn(E)).astype(np.float32)
         P[f + "layer_norm.bias"] = (0.1 * rs.randn(E)).astype(np.float32)
+    if rnn_cond == "film":
+        P = {k: v for k, v in P.items() if not k.startswith(d)}
+        P.update(_film_decoder_params(H, S, Z, seed))
+    return P
+
+
+def _film_decoder_params(H, S, Z, seed):
+    """RecurrentDecoderFiLM (modules.py:188-212): LinearNorm predictors (xavier-uniform weights), nn.Linear / nn.GRU default scales."""
+    rs = np.random.RandomState(seed + 7919)
+    d = "decoder.recurrent_decoder."
+    A, kb = P_IN + S, 1 / np.sqrt(H)
+    P = {}
+    for n in ("gammas", "betas"):
+        P[d + n + "_predictor.linear_layer.weight"] = _u(rs, (2 * H, Z), np.sqrt(6.0 / (Z + 2 * H)))
+        P[d + n + "_predictor.linear_layer.bias"] = _u(rs, (2 * H,), 1 / np.sqrt(Z))
+    P[d + "layer0.weight"] = _u(rs, (H, A), 1 / np.sqrt(A))
+    P[d + "layer0.bias"] = _u(rs, (H,), 1 / np.sqrt(A))
+    P[d + "layer1.weight_ih_l0"] = _u(rs, (3 * H, A + H), kb)
+    P[d + "layer1.weight_hh_l0"] = _u(rs, (3 * H, H), kb)
+    P[d + "layer1.bias_ih_l0"] = _u(rs, (3 * H,), kb)
+    P[d + "layer1.bias_hh_l0"] = _u(rs, (3 * H,), kb)
+    P[d + "layer1.weight_ih_l1"] = _u(rs, (3 * H, H), kb)
+    P[d + "layer1.weight_hh_l1"] = _u(rs, (3 * H, H), kb)
+    P[d + "layer1.bias_ih_l1"] = _u(rs, (3 * H,), kb)
+    P[d + "layer1.bias_hh_l1"] = _u(rs, (3 * H,), kb)
+    P[d + "layer2.weight"] = _u(rs, (H, H), kb)
+    P[d + "layer2.bias"] = _u(rs, (H,), kb)
+    P[d + "layer3.weight"] = _u(rs, (P_OUT, H), kb)
+    P[d + "layer3.bias"] = _u(rs, (P_OUT,), kb)
     return P
 
 

@@ -403,7 +403,7 @@ def build_networks(network_options, dimensions, style_encoding_type, nlabels, de
     se = modules.SpeechEncoder(dimensions["num_audio_features"], se_o["nhidden"], se_o["speech_encoding_size"]).to(device)
     de = modules.Decoder(pose_input_size=dimensions["pose_input_size"], pose_output_size=dimensions["pose_output_size"],
                          speech_encoding_size=se_o["speech_encoding_size"], style_encoding_size=Z,
-                         hidden_size=de_o["nhidden"], num_rnn_layers=2).to(device)
+                         hidden_size=de_o["nhidden"], num_rnn_layers=2, rnn_cond=de_o.get("rnn_cond", "normal")).to(device)
     st = None
     if style_encoding_type == "example":
         st = modules.StyleEncoder(dimensions["pose_input_size"], st_o["nhidden"], Z, type=st_o["type"],
