@@ -3,14 +3,16 @@
 the reference goldens (tests/golden/train_film_*.npz) and its graph replay / concurrent lanes against eager / one stream, and the
 tensor-core engine's refusal.
 
-Tolerances: forward 2e-3 x max(1, max|ref|) per pose-channel group (the fp32 engine's bound); gradients rel-L2 2e-3; train step as
-the fp32-engine rows of the train_h64 / train_h128 golden test (gemm mode 0)."""
+Tolerances: the fp32 engine's bounds of oracle/fp32_oracle.py -- forward FP32_FWD_TOL x max(1, max|ref|) per pose-channel group,
+gradients max-abs FP32_GEMM_GRAD_TOL x max|ref| (GEMM mode 1); train step as the fp32-engine rows of the train_h64 / train_h128 golden
+test (gemm mode 0)."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from oracle.fp32_oracle import FP32_FWD_TOL, FP32_GEMM_GRAD_TOL
 from tests._util import NAMES, ensure_built, stats_tensors, tt
 from tests.test_gpu_parity import _batch, _load
 
@@ -81,8 +83,8 @@ def test_film_window_forward_vs_oracle(dev, engine, H, B, T):
     for n, o, r in zip(NAMES, got, ref):
         err = float((o.cpu().double() - r).abs().max()) / max(1.0, float(r.abs().max()))
         worst = max(worst, err)
-        assert err <= 2e-3, (n, err)
-    print(f"  H={H} B={B} T={T}: worst per-group error {worst:.3e}")
+        assert err <= FP32_FWD_TOL, (n, err)
+    print(f"  H={H} B={B} T={T}: worst per-group error {worst:.3e} ({worst / FP32_FWD_TOL:.3f} of the bound)")
 
 
 @pytest.mark.parametrize("H", [64, 128, 1024])
@@ -114,11 +116,11 @@ def test_film_gradients_vs_oracle_autograd(dev, engine, H, B, T):
     ref = torch.autograd.grad(ref_loss, [Pd[k] for k in keys] + [sp, sy])
     bad, worst = [], 0.0
     for n, a, b in zip(names + ["dSpeech", "dStyle"], grads, ref):
-        e = float((a.cpu().double() - b).norm()) / max(float(b.norm()), 1e-30)
+        e = float((a.cpu().double() - b).abs().max()) / max(float(b.abs().max()), 1e-30)
         worst = max(worst, e)
-        if not e <= 2e-3:
+        if not e <= FP32_GEMM_GRAD_TOL:
             bad.append((n, e))
-    print(f"  H={H} B={B} T={T}: worst gradient rel-L2 {worst:.3e}")
+    print(f"  H={H} B={B} T={T}: worst gradient max-abs / max|ref| {worst:.3e} ({worst / FP32_GEMM_GRAD_TOL:.3f} of the bound)")
     assert not bad, bad
 
 

@@ -501,10 +501,19 @@ extern "C" size_t zeggs_decoder_bwd_workspace_bytes(int B, int T, int H, int S, 
 template <int U, bool FILM>
 static int launch_bwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdGeom& bg, const DecWs& w, const BwdWs& bw,
                       const BwdArgsDev& d, const FilmDev& f, cudaStream_t stream) {
-  size_t smem = (size_t)(8 * 2 * SkinnyCfg<4>::STG + 8 * 16 * 32 + 2 * g.nbt * U * 32 + g.nbt * bg.n4b * 16 * 32 + g.nbt * 9 * 32 + g.nbt * 7 * 32) * sizeof(float);
-  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int dev = 0, nsm = 0, occ = 0;
+  // dynamic shared memory per CTA: it grows with the 32-sample batch tiles, which bounds the batch of one call
+  auto smem_of = [&](int nbt) {
+    return (size_t)(8 * 2 * SkinnyCfg<4>::STG + 8 * 16 * 32 + 2 * nbt * U * 32 + nbt * bg.n4b * 16 * 32 + nbt * 9 * 32 + nbt * 7 * 32) * sizeof(float);
+  };
+  const size_t smem = smem_of(g.nbt);
+  int dev = 0, nsm = 0, occ = 0, cap = 0;
   ZCHECK_CUDA(cudaGetDevice(&dev));
+  ZCHECK_CUDA(cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  int max_nbt = g.nbt;
+  while (max_nbt > 0 && smem_of(max_nbt) > (size_t)cap) --max_nbt;
+  ZCHECK_ARG(smem <= (size_t)cap, "decoder bwd: batch %d needs %zu bytes of shared memory per CTA at hidden size %d (%d available): at most "
+             "%d samples per call", g.B, smem, g.H, cap, 32 * max_nbt);
+  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
   ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_bwd_kernel<U, FILM>, 256, smem));
   ZCHECK_ARG(occ * nsm >= g.G, "decoder bwd: cooperative grid of %d CTAs does not fit", g.G);
@@ -566,8 +575,10 @@ int wgrad_gemms(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b
   const int H = a.H, A = g.A, C = a.S + a.Z;
   const int cur = g.nbt * 32;                       // column offset of slot t = 1
   const int Kc = (a.T - 1) * g.nbt * 32;
+  char* const end = scratch_base() + scratch_bytes();
   char* ws_p = (char*)(((uintptr_t)tail + 255) & ~(uintptr_t)255);
-  const size_t ws_bytes = (size_t)(scratch_base() + scratch_bytes() - ws_p);
+  // the histories may end within 255 bytes of the scratch end: the aligned tail then lies past it and there is no split-K room
+  const size_t ws_bytes = ws_p < end ? (size_t)(end - ws_p) : 0;
   auto G = [&](int ga, int ga_off, int N, int xb, int xb_off, int K, float* dW, int ldw) {
     const WgradHist &x = hs.h[ga], &y = hs.h[xb];
     return tc_gemm_launch(N, K, Kc, x.hi + ga_off, want_lo ? x.lo + ga_off : nullptr, (int)hs.ld,

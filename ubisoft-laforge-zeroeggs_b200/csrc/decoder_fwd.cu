@@ -325,11 +325,29 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
 }
 
 // ------------------------------------------------------------------ host side
+// dynamic shared memory per CTA of the fp32 recurrence: it grows with the 32-sample batch tiles, which bounds the batch of one call
+template <int U>
+static size_t fwd_smem_bytes(int nbt) {
+  constexpr int RT2 = (6 * U) / 4;
+  return (size_t)(8 * 2 * SkinnyCfg<RT2>::STG + 8 * 6 * U * 32 + nbt * 3 * U * 32 + 6 * 32) * sizeof(float);
+}
+
 static int check_fwd_args(const zeggs_decoder_fwd_args* a) {
   ZCHECK_ARG(a != nullptr, "decoder: null args");
   ZCHECK_ARG(a->B >= 1 && a->T >= 1, "decoder: bad B=%d T=%d", a->B, a->T);
   ZCHECK_ARG(a->H % 16 == 0 && pick_U(a->H) > 0, "decoder: hidden size %d unsupported (need H%%16==0, H<=1056)", a->H);
   ZCHECK_ARG(a->S >= 1 && a->Z >= 1 && a->S + a->Z <= 256, "decoder: bad S=%d Z=%d", a->S, a->Z);
+  if (a->engine != 1) {
+    size_t (*smem_of)(int) = pick_U(a->H) == 4 ? fwd_smem_bytes<4> : fwd_smem_bytes<8>;
+    const int nbt = ceil_div(a->B, 32);
+    int dev = 0, cap = 0;
+    ZCHECK_CUDA(cudaGetDevice(&dev));
+    ZCHECK_CUDA(cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    int max_nbt = nbt;
+    while (max_nbt > 0 && smem_of(max_nbt) > (size_t)cap) --max_nbt;
+    ZCHECK_ARG(smem_of(nbt) <= (size_t)cap, "decoder: batch %d needs %zu bytes of shared memory per CTA at hidden size %d (%d available): at "
+               "most %d samples per call", a->B, smem_of(nbt), a->H, cap, 32 * max_nbt);
+  }
   return ZEGGS_OK;
 }
 
@@ -358,8 +376,7 @@ extern "C" size_t zeggs_decoder_workspace_bytes(int B, int T, int H, int S, int 
 
 template <int U, bool FILM>
 static int launch_fwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, const FilmDev& f, cudaStream_t stream) {
-  constexpr int RT2 = (6 * U) / 4;
-  size_t smem = (size_t)(8 * 2 * SkinnyCfg<RT2>::STG + 8 * 6 * U * 32 + g.nbt * 3 * U * 32 + 6 * 32) * sizeof(float);
+  const size_t smem = fwd_smem_bytes<U>(g.nbt);            // within the device's limit: check_fwd_args
   ZCHECK_CUDA(cudaFuncSetAttribute(decoder_fwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int dev = 0, nsm = 0, occ = 0;
   ZCHECK_CUDA(cudaGetDevice(&dev));
