@@ -13,6 +13,7 @@ from pathlib import Path
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib, dp, modules, ops
 from .optimizers import RAdam
@@ -413,8 +414,12 @@ def build_networks(network_options, dimensions, style_encoding_type, nlabels, de
 
 def train(models_dir, logs_dir, path_processed_data, path_data_definition, train_options, network_options):
     """Drop-in for ZEGGS/train.py:29 (same arguments, same artefacts in models_dir).  Data-parallel when launched under
-    torchrun (RANK/WORLD_SIZE set): each rank draws its own windows, one gradient all-reduce per step."""
+    torchrun (RANK/WORLD_SIZE set): each rank draws its own windows, one gradient all-reduce per step.  With `use_tensorboard`,
+    rank 0 also writes logs_dir/tb (TensorBoardLog) from the loss terms every rank collects (LossLog)."""
     from .data import DevicePrefetcher, DeviceWindowDataset, WindowDataset
+    use_tb = bool(train_options.get("use_tensorboard", False))
+    if use_tb:
+        summary_writer_class()               # a missing tensorboard package fails here, before any work, as the reference's import does
     np.random.seed(train_options["seed"])
     torch.manual_seed(train_options["seed"])
     if not (train_options["use_gpu"] and torch.cuda.is_available()):
@@ -462,6 +467,10 @@ def train(models_dir, logs_dir, path_processed_data, path_data_definition, train
         samples_dir.mkdir(parents=True, exist_ok=True)
     prefetch = None if on_device else DevicePrefetcher(device)
     token = None if on_device else prefetch.upload(ds.sample_host_batch(batchsize))
+    # every rank collects (under data parallelism the blocks are averaged over ranks); rank 0 writes
+    losslog = LossLog(device, group=stepper.pg) if use_tb else None
+    tb = TensorBoardLog(logs_dir / "tb", network_options, train_options) if use_tb and rank == 0 else None
+    log = (lambda steps, rows: tb.write("losses", steps, rows)) if tb is not None else (lambda steps, rows: None)
     while stepper.iteration < total:
         if on_device:
             batch = ds.sample_batch(batchsize)                                        # one gather launch out of the HBM-resident arrays
@@ -472,24 +481,33 @@ def train(models_dir, logs_dir, path_processed_data, path_data_definition, train
             token = prefetch.upload(ds.sample_host_batch(batchsize))                  # next step's windows copy under this step
         loss = stepper.step(batch)
         it = stepper.iteration
+        if losslog is not None:
+            log(*losslog.push(stepper))           # before the progress line's .item(): the writing overlaps the queued steps
         if it % 1000 == 0:
             for g in stepper.optimizer.param_groups:
                 g["lr"] *= decay                                                     # ExponentialLR every 1000 its (:431-432)
         if rank == 0 and (it % 100 == 0 or it == 1):
             print(f"iteration {it}/{total} loss {loss.item():.5f} elapsed {datetime.datetime.now() - start}", flush=True)
+        if losslog is not None and it % train_options["generate_samples_step"] == 0:
+            log(*losslog.drain())                 # on every rank: a collective under data parallelism
         if rank == 0 and it % train_options["generate_samples_step"] == 0:
             train_loss = float(loss.item())
             save_checkpoint(models_dir, se, de, st, stepper, train_loss)
             save_checkpoint(models_dir / str(it), se, de, st, stepper, train_loss)             # train.py:493-509
             monitor(stepper, ds, batchsize, it, train_loss, logs_dir, samples_dir, se, de, st, details, style_encoding_type,
-                    sample_rs, device)
+                    sample_rs, device, tb=tb)
+    if losslog is not None:
+        log(*losslog.drain())
     if rank == 0:
         save_checkpoint(models_dir, se, de, st, stepper, float(loss.item()))
+    if tb is not None:
+        tb.close()
 
 
-def monitor(stepper, ds, batchsize, it, train_loss, logs_dir, samples_dir, se, de, st, details, style_encoding_type, rs, device):
+def monitor(stepper, ds, batchsize, it, train_loss, logs_dir, samples_dir, se, de, st, details, style_encoding_type, rs, device, tb=None):
     """What train() does at every generate_samples_step besides saving: the sample animations (train.py:511-729) and the held-out
-    loss (validate), printed and appended as one JSON line to logs_dir/valid_loss.jsonl.  Touches nothing the training reads."""
+    loss (validate), printed and appended as one JSON line to logs_dir/valid_loss.jsonl, and written as `valid/*` at step `it` to
+    the TensorBoardLog `tb` if given.  Touches nothing the training reads."""
     has_valid = len(ds.ranges_valid) > 0
     write_samples(samples_dir, it, ds, se, de, st, ds.stats, details, style_encoding_type, rs, device,
                   splits=("train", "valid") if has_valid else ("train",))
@@ -503,6 +521,108 @@ def monitor(stepper, ds, batchsize, it, train_loss, logs_dir, samples_dir, se, d
             fh.write(json.dumps(rec) + "\n")
     except (PermissionError, OSError) as e:
         print(e)
+    if tb is not None:
+        tb.write("valid", [it], terms[None].astype(np.float32))
+
+
+def flatten_options(d, prefix=""):
+    """Nested option dicts -> one flat dict whose keys join the path with "_" ({"decoder": {"nhidden": 1024}} -> {"decoder_nhidden":
+    1024}), the hyper-parameter names the reference's TensorBoard run carries (helpers.py:14-23)."""
+    out = {}
+    for k, v in d.items():
+        key = f"{prefix}_{k}" if prefix else k
+        if isinstance(v, dict):
+            out.update(flatten_options(v, key))
+        else:
+            out[key] = v
+    return out
+
+
+def summary_writer_class():
+    """torch.utils.tensorboard.SummaryWriter, or ZeggsError when the tensorboard package is missing."""
+    try:
+        from torch.utils.tensorboard import SummaryWriter
+    except ImportError as e:
+        raise _lib.ZeggsError(f"use_tensorboard is set but torch.utils.tensorboard cannot be imported ({e}): install the tensorboard "
+                              "package or set use_tensorboard to false") from e
+    return SummaryWriter
+
+
+class TensorBoardLog:
+    """The reference's TensorBoard run (train.py:179-187, 437-463) in directory `tb_dir`: the flattened network and training options as
+    hyper-parameters once, then per step `<prefix>/total_loss` and `<prefix>/losses` with the 18 named terms (`loss_root_pos` ...
+    `loss_gaze`, `loss_kl_div` = the weighted KL), one sub-run per term (tb/<prefix>_losses_loss_*/) as add_scalars lays them out.
+    train() writes prefix "losses" for every optimizer step and "valid" for the held-out loss."""
+
+    def __init__(self, tb_dir, network_options, train_options):
+        self.writer = summary_writer_class()(str(tb_dir), flush_secs=10)
+        h = flatten_options(network_options)
+        h.update(flatten_options(train_options))
+        self.writer.add_hparams(h, {"No Metric": 0.0})
+
+    def write(self, prefix, steps, rows):
+        """rows[i] (the 19 TERM_NAMES values) at step steps[i]."""
+        for s, r in zip(steps, rows):
+            s = int(s)
+            self.writer.add_scalar(f"{prefix}/total_loss", r[0], s)
+            self.writer.add_scalars(f"{prefix}/losses", {"loss_" + n: r[j] for j, n in enumerate(TERM_NAMES[1:], 1)}, s)
+
+    def close(self):
+        self.writer.close()
+
+
+class LossLog:
+    """Every step's 19 loss terms (TrainStep.terms) brought to the host without a per-step device sync.  `push(stepper)` after each
+    step enqueues one device-to-device copy of the terms into the next row of a [block, 19] device history, on the current stream:
+    behind the step that wrote them, ahead of the next one that overwrites them.  When a block fills, its rows are averaged over the
+    ranks of `group` (one all-reduce per block; exact, since every term is a batch mean and the per-rank batches are equal) and
+    copied to pinned host memory behind an event; the PREVIOUS block's rows, long landed, are returned then.  So a push that does
+    not fill a block returns nothing and waits for nothing, and the host gets the rows at most two blocks late.  `drain()` closes the
+    open block, waits and returns everything pending; under data parallelism every rank must push and drain at the same steps.
+    Both return (steps int64 [n], rows float32 [n, 19]); a row's step is stepper.iteration - 1, the 0-based optimizer step."""
+
+    def __init__(self, device, block=100, group=None):
+        self.dev = torch.device(device)
+        self.group = group
+        self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+        self.hist = torch.zeros(block, 19, dtype=torch.float32, device=self.dev)
+        self.host = torch.zeros(block, 19, dtype=torch.float32).pin_memory()
+        self.steps = []                # steps of the rows in the open block
+        self.pending = None            # (steps, event) of the closed block whose copy to `host` is in flight
+
+    def push(self, stepper):
+        self.hist[len(self.steps)].copy_(stepper.terms, non_blocking=True)
+        self.steps.append(stepper.iteration - 1)
+        if len(self.steps) < self.hist.shape[0]:
+            return np.zeros(0, np.int64), np.zeros((0, 19), np.float32)
+        return self._close()
+
+    def drain(self):
+        s0, r0 = self._close()
+        s1, r1 = self._collect()
+        return np.concatenate([s0, s1]), np.concatenate([r0, r1])
+
+    def _collect(self):
+        if self.pending is None:
+            return np.zeros(0, np.int64), np.zeros((0, 19), np.float32)
+        steps, ev = self.pending
+        self.pending = None
+        ev.synchronize()
+        return np.asarray(steps, np.int64), self.host[:len(steps)].numpy().copy()
+
+    def _close(self):
+        out = self._collect()                  # before the next copy into `host`
+        n = len(self.steps)
+        if n:
+            rows = self.hist[:n]
+            if self.world > 1:
+                dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=self.group)
+                rows.mul_(1.0 / self.world)
+            self.host[:n].copy_(rows, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(self.dev))
+            self.pending, self.steps = (self.steps, ev), []
+        return out
 
 
 def save_checkpoint(models_dir, se, de, st, stepper, loss):
