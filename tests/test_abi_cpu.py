@@ -57,6 +57,30 @@ def test_workspace_and_pack_sizes(built):
     assert a > b > 0
 
 
+def test_style_gru_refuses_batches_its_backward_cannot_hold(built):
+    """The GRU encoder's BPTT kernel keeps a carry of U*32 floats per 32-sample tile in shared memory, so at H = 1056 (U = 8) one call
+    takes at most 1216 samples on an H100 (227 KB per block).  The workspace query reports 0 and both entry points refuse a larger
+    batch, naming the limit, before they launch anything (before, the backward failed at cudaFuncSetAttribute after the forward ran)."""
+    import ctypes
+    l = built.lib()
+    assert l.zeggs_style_enc_gru_workspace_bytes(1216, 17, 1134, 1056, 128, 1) > 0
+    assert l.zeggs_style_enc_gru_workspace_bytes(1217, 17, 1134, 1056, 128, 1) == 0
+    assert l.zeggs_style_enc_gru_workspace_bytes(7936, 17, 1134, 528, 128, 1) > 0        # U = 4: 248 tiles
+    assert l.zeggs_style_enc_gru_workspace_bytes(7937, 17, 1134, 528, 128, 1) == 0
+    assert l.zeggs_style_enc_gru_workspace_bytes(1, 17, 1134, 532, 128, 1) == 0          # unsupported hidden size
+    dummy = ctypes.create_string_buffer(64)
+    p = ctypes.addressof(dummy)
+    a = built.StyleEncGruArgs(B=1217, T=17, C_in=1134, H=1056, E=128, temperature=1.0, x=p, z=p, mu=p, logvar=p, workspace=p,
+                              workspace_bytes=1 << 40)
+    g = built.StyleEncGruGrads(dz=p, dmu=p, dlogvar=p)
+    launches = l.zeggs_launch_count()
+    assert l.zeggs_style_enc_gru_fwd(ctypes.byref(a), None) != 0
+    assert "at most 1216 samples" in l.zeggs_last_error().decode()
+    assert l.zeggs_style_enc_gru_bwd(ctypes.byref(a), ctypes.byref(g), None) != 0
+    assert "at most 1216 samples" in l.zeggs_last_error().decode()
+    assert l.zeggs_launch_count() == launches
+
+
 def test_host_filterbank_matches_oracle():
     from oracle import mel_oracle
     from zeggs_b200.audio import mel_filterbank

@@ -53,6 +53,7 @@ int sgemm_batched2_launch(int mode, int M, int N, int K, const float* A, int lda
                           float alpha, cudaStream_t stream);
 // StyleEncoderGRU recurrences (style_gru.cu)
 int style_gru_units(int H);
+int style_gru_max_batch(int H);
 int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
                          unsigned* bar, cudaStream_t s);
 int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs, const float* Gs, const float* dhf, int ld_dhf,

@@ -515,7 +515,8 @@ static StyleGruWs style_gru_ws(void* base, int B, int T, int Cin, int H, int E, 
   w.bytes = a.off; return w;
 }
 extern "C" size_t zeggs_style_enc_gru_workspace_bytes(int B, int T, int Cin, int H, int E, int use_vae) {
-  if (B < 1 || T < 1 || Cin < 1 || E < 1 || style_gru_units(H) == 0 || (use_vae && E % 2)) return 0;
+  // style_gru_max_batch is 0 for an unsupported hidden size
+  if (B < 1 || T < 1 || Cin < 1 || E < 1 || B > style_gru_max_batch(H) || (use_vae && E % 2)) return 0;
   return style_gru_ws(nullptr, B, T, Cin, H, E, use_vae != 0).bytes;
 }
 
@@ -528,6 +529,8 @@ extern "C" int zeggs_style_enc_gru_fwd(const zeggs_style_enc_gru_args* ap, void*
   ZCHECK_ARG(B >= 1 && T >= 1 && Cin >= 1 && E >= 1 && (!vae || E % 2 == 0) && a.x && a.z && (a.logvar != nullptr) == vae,
              "style_enc_gru: bad arguments");
   ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru: hidden size %d unsupported (H %% 4 == 0 and H <= 528, or H %% 8 == 0 and H <= 1056)", H);
+  ZCHECK_ARG(B <= style_gru_max_batch(H), "style_enc_gru: batch %d too large: at hidden size %d the backward's shared memory holds at "
+             "most %d samples per call", B, H, style_gru_max_batch(H));
   StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);
   ZCHECK_ARG(a.workspace && a.workspace_bytes >= w.bytes, "style_enc_gru: workspace too small");
   ScopedTimer tm("encoders_fwd", s);
@@ -555,6 +558,8 @@ extern "C" int zeggs_style_enc_gru_bwd(const zeggs_style_enc_gru_args* ap, const
   const bool vae = a.mu != nullptr;
   ZCHECK_ARG(vae || (g.dz && !g.dmu && !g.dlogvar), "style_enc_gru bwd: without the VAE (mu == NULL) dz [B,E] is required and dmu / dlogvar must be NULL");
   ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru bwd: hidden size %d unsupported", H);
+  ZCHECK_ARG(B <= style_gru_max_batch(H), "style_enc_gru bwd: batch %d too large: at hidden size %d the shared memory holds at most %d "
+             "samples per call", B, H, style_gru_max_batch(H));
   StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);
   ZCHECK_ARG(a.workspace && a.workspace_bytes >= w.bytes, "style_enc_gru bwd: workspace too small");
   g_redbuf = w.red;

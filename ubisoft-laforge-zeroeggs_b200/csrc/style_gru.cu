@@ -51,9 +51,23 @@ int style_gru_units(int H) {
   return 0;
 }
 
+// dynamic shared memory per CTA: the forward kernel's with nbt = 0, the BPTT kernel's with its nbt 32-sample tiles of carry
 template <int U>
 static size_t gru_smem_bytes(int H, int nbt) {
   return (size_t)(3 * U * H + GRU_KC * 33 + 8 * 3 * U * 32 + nbt * U * 32) * sizeof(float);
+}
+
+// The opt-in shared memory of one block on sm_90 (227 KB).  A constant rather than a device query, so the workspace query and
+// both entry points refuse a batch the backward cannot run before the forward has run.
+constexpr size_t GRU_SMEM_LIMIT = 232448;
+
+// the largest batch one call takes at hidden size H (0 = H unsupported): the BPTT kernel's carry grows by U*32 floats per tile
+int style_gru_max_batch(int H) {
+  const int U = style_gru_units(H);
+  if (U == 0) return 0;
+  int nbt = 0;
+  while ((U == 4 ? gru_smem_bytes<4>(H, nbt + 1) : gru_smem_bytes<8>(H, nbt + 1)) <= GRU_SMEM_LIMIT) ++nbt;
+  return 32 * nbt;
 }
 
 // ------------------------------------------------------------------ forward recurrence (modules.py:341, nn.GRU gate order r, z, n)
@@ -275,6 +289,8 @@ int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs,
                          float* dGih, float* dGhh, unsigned* bar, cudaStream_t s) {
   const int U = style_gru_units(H);
   ZCHECK_ARG(U > 0 && B >= 1 && T >= 1, "style GRU: hidden size %d unsupported", H);
+  ZCHECK_ARG(B <= style_gru_max_batch(H), "style GRU bwd: batch %d above the %d samples the shared memory holds at hidden size %d", B,
+             style_gru_max_batch(H), H);
   ZCHECK_CUDA(cudaMemsetAsync(bar, 0, 2 * sizeof(unsigned), s));
   const int nbt = (B + 31) / 32;
   void* args[] = {(void*)&B, (void*)&T, (void*)&H, (void*)&Whh, (void*)&Hs, (void*)&Gs, (void*)&dhf, (void*)&ld_dhf, (void*)&dGih,

@@ -633,9 +633,8 @@ def style_encoder_fwd(enc, x, eps, masks, temperature):
     if enc.encoder_type == "gru":
         H, E = weights[0].shape[0], weights[12].shape[0]
         outs = _style_outputs(enc, B, E, x.device)
+        # 0 bytes when the library refuses the shape (hidden size, odd encoding with the VAE, batch): the call below says why
         nb = l.zeggs_style_enc_gru_workspace_bytes(B, T, Cin, H, E, int(bool(enc.use_vae)))
-        if nb == 0:
-            raise _lib.ZeggsError(f"GRU style encoder: hidden size {H} / encoding size {E} unsupported")
         ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
         a, keep = style_gru_args(enc, x, eps, temperature, outs, ws)
         _lib.check(l.zeggs_style_enc_gru_fwd(a, _lib.stream_ptr()), "zeggs_style_enc_gru_fwd")
