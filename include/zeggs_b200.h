@@ -121,6 +121,8 @@ int zeggs_loudness_gain(const zeggs_loudness_args* a, void* stream);
 /* ------------------------------------------------------------------------------------------------
  * Decoder (modules.py:11-243, 677-742): CellStateEncoder + T-1 autoregressive steps of
  * vectorize_input -> Linear+ELU -> 2-layer GRU -> Linear -> devectorize_output, one persistent kernel.
+ * Supported hidden sizes: engine 0 (and the FiLM decoder) H % 16 == 0 and H <= 2112 (H/U CTAs, U = 4 up to 528, 8 up to 1056, 16
+ * above); engine 1 H % 128 == 0 and 384 <= H <= 1024.  Every size / pack / workspace query returns 0 outside the engine-0 rule.
  */
 typedef struct {
   int B, T, H, S, Z; /* batch, frames, hidden (modules.py:18), speech / style encoding sizes */

@@ -15,29 +15,32 @@
 
 namespace zeggs {
 
-// PB1[c][k<1136][R1]      W2[k][cU+r]                       (x = dy, k = output channel)
-// PB2[c][k<3H][2U]        r<U: W_ih1[k][cU+r]   else W_hh1[k][cU+r-U]
-// PB3a[c][k<3H][2U]       r<U: W_ih0[k][cU+r]   else W_hh0[k][cU+r-U]
+// CTA c's units are passes p of V = pass_units(U) units (one pass below U = 16); j(r) = cU + pV + r, R1P = film_rows(V) = R1 / (U/V):
+// PB1[c][p][k<1136][R1P]  W2[k][j(r)]                       (x = dy, k = output channel)
+// PB2[c][p][k<3H][2V]     r<V: W_ih1[k][j(r)]   else W_hh1[k][j(r-V)]
+// PB3a[c][p][k<3H][2V]    r<V: W_ih0[k][j(r)]   else W_hh0[k][j(r-V)]
 // PB3b[c][tile][k<3H][16] W_ih0[k][H + perm(c*rpcb + tile*16 + r)]
 // PB4[c][tile][k<H][16]   W0[k][perm(c*rpcb + tile*16 + r)]
 __global__ void pack_decoder_bwd_kernel(DecGeom g, BwdGeom bg, const float* __restrict__ W0, const float* __restrict__ Wih0,
                                         const float* __restrict__ Whh0, const float* __restrict__ Wih1,
                                         const float* __restrict__ Whh1, const float* __restrict__ W2, float* __restrict__ out) {
-  const int H = g.H, U = g.U, A = g.A;
+  const int H = g.H, U = g.U, A = g.A, V = pass_units(U), NP = U / V, R1P = bg.R1 / NP;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < bg.total; i += (size_t)gridDim.x * blockDim.x) {
     float v = 0.f;
     if (i < bg.off2) {
       size_t e = i;
-      int r = e % bg.R1; e /= bg.R1;
-      int k = e % K1P; int c = e / K1P;
-      if (r < U && k < P_OUT) v = W2[(size_t)k * H + c * U + r];
+      int r = e % R1P; e /= R1P;
+      int k = e % K1P; e /= K1P;
+      int p = e % NP, c = e / NP;
+      if (r < V && k < P_OUT) v = W2[(size_t)k * H + c * U + p * V + r];
     } else if (i < bg.off3b) {
       const bool l0 = i >= bg.off3a;
       size_t e = i - (l0 ? bg.off3a : bg.off2);
-      int r = e % (2 * U); e /= (2 * U);
-      int k = e % (3 * H); int c = e / (3 * H);
-      const bool hh = r >= U;
-      int j = c * U + (hh ? r - U : r);
+      int r = e % (2 * V); e /= (2 * V);
+      int k = e % (3 * H); e /= (3 * H);
+      int p = e % NP, c = e / NP;
+      const bool hh = r >= V;
+      int j = c * U + p * V + (hh ? r - V : r);
       if (!l0) v = hh ? Whh1[(size_t)k * H + j] : Wih1[(size_t)k * H + j];
       else     v = hh ? Whh0[(size_t)k * H + j] : Wih0[(size_t)k * (A + H) + j];
     } else {
@@ -59,12 +62,14 @@ __global__ void pack_decoder_bwd_kernel(DecGeom g, BwdGeom bg, const float* __re
 
 // FILM: the FiLM decoder's BPTT.  B1 splits in two stages: B1a  dc = W3^T (dY_acc*sigma_out) -> d gamma/beta of layer2, dpre2 (DP2);
 // B1b  dh1 = dh1_acc + Wm^T dpre2.  B3 takes the layer-0 modulation: d gamma/beta of layer0, dpre_a = da * gamma * ELU'.
+// B1 / B1a / B2 / B3a run once per pass of V units, on the pass-major slices PB1 / PBm / PB2 / PB3a.
 template <int U, bool FILM>
 __global__ void __launch_bounds__(256, 1)
 decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, BwdWs bw, BwdArgsDev d, FilmDev f) {
   extern __shared__ __align__(16) float smem[];
-  constexpr int RT1 = (U < 8 ? 8 : U) / 4;   // B1 tile rows / 4
-  constexpr int RT2 = (2 * U) / 4;           // dual tiles
+  constexpr int V = pass_units(U), NP = U / V;
+  constexpr int RT1 = film_rows(V) / 4;      // B1 tile rows / 4
+  constexpr int RT2 = (2 * V) / 4;           // dual tiles
   constexpr int RTM = 4;                     // widest tile used here (16 rows)
   float* stage = smem;                                   // 8 warps x 2 x STG(RTM)
   float* red = smem + 8 * 2 * SkinnyCfg<RTM>::STG;       // [8][16][32]
@@ -78,11 +83,11 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
   float* wstage = stage + warp * 2 * SkinnyCfg<RTM>::STG;
   GridBarrier gb; gb.counter = bw.bar; gb.error = bw.bar + 1; gb.epoch = 0; gb.nblocks = gridDim.x;
   const float* PB1 = d.packed + (size_t)c * K1P * bg.R1;
-  const float* PB2 = d.packed + bg.off2 + (size_t)c * 3 * H * 2 * U;
+  const float* PB2 = d.packed + bg.off2 + (size_t)c * 3 * H * 2 * U;    // + p * 3H * 2V per pass
   const float* PB3a = d.packed + bg.off3a + (size_t)c * 3 * H * 2 * U;
   const float* PB3b = d.packed + bg.off3b + (size_t)c * bg.n4b * 3 * H * 16;
   const float* PB4 = d.packed + bg.off4 + (size_t)c * bg.n4b * H * 16;
-  const float* PBm = d.packed + bg.total + (size_t)c * H * bg.R1;   // FiLM: PBm[c][k][r] = Wm[k][c*U + r]
+  const float* PBm = d.packed + bg.total + (size_t)c * H * bg.R1;   // FiLM: PBm[c][p][k][r] = Wm[k][c*U + p*V + r]
   const size_t actH = (size_t)nbt * H * 32, act3 = (size_t)nbt * 3 * H * 32, actX = (size_t)nbt * K1P * 32, act4 = (size_t)nbt * 4 * H * 32;
 
   // R(t): finalise dY_acc[t] from dxp (shared `red`-summed values passed through `dxpv`), write DY[t] (scaled by sigma_out).
@@ -178,15 +183,16 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
   for (int t = T - 1; t >= 1; --t) {
     if constexpr (FILM) {
       // ---------------------------------------------------------- B1a (FiLM: layer3, modulation and ELU of layer2)
-      for (int bt = 0; bt < nbt; ++bt) {
+      for (int bt = 0; bt < nbt; ++bt)
+      for (int p = 0; p < NP; ++p) {
         float acc[RT1][4];
         const float* x = bw.DY + t * actX + (size_t)bt * K1P * 32;
-        skinny_gemm<RT1, false>(acc, PB1, x, x, K1P / 16, wstage);
+        skinny_gemm<RT1, false>(acc, PB1 + (size_t)p * K1P * 4 * RT1, x, x, K1P / 16, wstage);
         reduce_store<RT1>(acc, red);
         __syncthreads();
-        for (int idx = tid; idx < U * 32; idx += 256) {
-          const int u = idx >> 5, b = idx & 31, j = c * U + u, bgl = bt * 32 + b;
-          const float dc = red_sum<4 * RT1>(red, u, b);
+        for (int idx = tid; idx < V * 32; idx += 256) {
+          const int b = idx & 31, j = c * U + p * V + (idx >> 5), bgl = bt * 32 + b;
+          const float dc = red_sum<4 * RT1>(red, idx >> 5, b);
           const float e = f.E2[t * actH + ((size_t)bt * H + j) * 32 + b];
           float gm = 1.f;
           if (bgl < a.B) {
@@ -202,21 +208,22 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
       if (!grid_sync(gb)) return;
     }
     // ------------------------------------------------------------ B1 (FiLM: B1b)
-    for (int bt = 0; bt < nbt; ++bt) {
+    for (int bt = 0; bt < nbt; ++bt)
+    for (int p = 0; p < NP; ++p) {
       float acc[RT1][4];
       if constexpr (FILM) {
         const float* x = f.DP2 + t * actH + (size_t)bt * H * 32;
-        skinny_gemm<RT1, false>(acc, PBm, x, x, H / 16, wstage);
+        skinny_gemm<RT1, false>(acc, PBm + (size_t)p * H * 4 * RT1, x, x, H / 16, wstage);
       } else {
         const float* x = bw.DY + t * actX + (size_t)bt * K1P * 32;
-        skinny_gemm<RT1, false>(acc, PB1, x, x, K1P / 16, wstage);
+        skinny_gemm<RT1, false>(acc, PB1 + (size_t)p * K1P * 4 * RT1, x, x, K1P / 16, wstage);
       }
       reduce_store<RT1>(acc, red);
       __syncthreads();
-      for (int idx = tid; idx < U * 32; idx += 256) {
-        const int u = idx >> 5, b = idx & 31, j = c * U + u;
+      for (int idx = tid; idx < V * 32; idx += 256) {
+        const int u = p * V + (idx >> 5), b = idx & 31, j = c * U + u;
         float* acc1 = bw.DH1 + ((size_t)bt * H + j) * 32 + b;
-        float dh = red_sum<4 * RT1>(red, u, b) + (t == T - 1 ? 0.f : *acc1);
+        float dh = red_sum<4 * RT1>(red, idx >> 5, b) + (t == T - 1 ? 0.f : *acc1);
         const float* G = w.G1 + t * act4 + (size_t)bt * 4 * H * 32;
         float r = G[(size_t)(0 * H + j) * 32 + b], z = G[(size_t)(1 * H + j) * 32 + b];
         float n = G[(size_t)(2 * H + j) * 32 + b], ghn = G[(size_t)(3 * H + j) * 32 + b];
@@ -234,17 +241,18 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
     }
     if (!grid_sync(gb)) return;
     // ------------------------------------------------------------ B2
-    for (int bt = 0; bt < nbt; ++bt) {
+    for (int bt = 0; bt < nbt; ++bt)
+    for (int p = 0; p < NP; ++p) {
       float acc[RT2][4];
       const float* xa = bw.DGI1 + t * act3 + (size_t)bt * 3 * H * 32;
       const float* xb = bw.DGH1 + t * act3 + (size_t)bt * 3 * H * 32;
-      skinny_gemm<RT2, true>(acc, PB2, xa, xb, 3 * H / 16, wstage);
+      skinny_gemm<RT2, true>(acc, PB2 + (size_t)p * 3 * H * 2 * V, xa, xb, 3 * H / 16, wstage);
       reduce_store<RT2>(acc, red);
       __syncthreads();
-      for (int idx = tid; idx < U * 32; idx += 256) {
-        const int u = idx >> 5, b = idx & 31, j = c * U + u;
+      for (int idx = tid; idx < V * 32; idx += 256) {
+        const int u = p * V + (idx >> 5), v = idx >> 5, b = idx & 31, j = c * U + u;
         float* acc0 = bw.DH0 + ((size_t)bt * H + j) * 32 + b;
-        float dh = red_sum<2 * U>(red, u, b) + (t == T - 1 ? 0.f : *acc0);
+        float dh = red_sum<2 * V>(red, v, b) + (t == T - 1 ? 0.f : *acc0);
         const float* G = w.G0 + t * act4 + (size_t)bt * 4 * H * 32;
         float r = G[(size_t)(0 * H + j) * 32 + b], z = G[(size_t)(1 * H + j) * 32 + b];
         float n = G[(size_t)(2 * H + j) * 32 + b], ghn = G[(size_t)(3 * H + j) * 32 + b];
@@ -258,24 +266,24 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
           bw.DGH0[t * act3 + ((size_t)bt * 3 * H + q * H + j) * 32 + b] = dgh[q];
         }
         // dh1(t-1) = dh1*z1 + W_hh1^T dgh1
-        bw.DH1[((size_t)bt * H + j) * 32 + b] = red_sum<2 * U>(red, U + u, b) + dhz1[(bt * U + u) * 32 + b];
+        bw.DH1[((size_t)bt * H + j) * 32 + b] = red_sum<2 * V>(red, V + v, b) + dhz1[(bt * U + u) * 32 + b];
       }
       __syncthreads();
     }
     if (!grid_sync(gb)) return;
     // ------------------------------------------------------------ B3
     for (int bt = 0; bt < nbt; ++bt) {
-      {
+      for (int p = 0; p < NP; ++p) {
         float acc[RT2][4];
         const float* xa = bw.DGI0 + t * act3 + (size_t)bt * 3 * H * 32;
         const float* xb = bw.DGH0 + t * act3 + (size_t)bt * 3 * H * 32;
-        skinny_gemm<RT2, true>(acc, PB3a, xa, xb, 3 * H / 16, wstage);
+        skinny_gemm<RT2, true>(acc, PB3a + (size_t)p * 3 * H * 2 * V, xa, xb, 3 * H / 16, wstage);
         reduce_store<RT2>(acc, red);
         __syncthreads();
-        for (int idx = tid; idx < U * 32; idx += 256) {
-          const int u = idx >> 5, b = idx & 31, j = c * U + u;
+        for (int idx = tid; idx < V * 32; idx += 256) {
+          const int u = p * V + (idx >> 5), v = idx >> 5, b = idx & 31, j = c * U + u;
           if constexpr (FILM) {
-            const float da = red_sum<2 * U>(red, u, b);
+            const float da = red_sum<2 * V>(red, v, b);
             const int bgl = bt * 32 + b;
             const float e = f.E0[t * actH + ((size_t)bt * H + j) * 32 + b];
             float gm = 1.f;
@@ -288,10 +296,10 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
             bw.DPA[t * actH + ((size_t)bt * H + j) * 32 + b] = da * gm * (e > 0.f ? 1.f : e + 1.f);
           } else {
             float av = w.A[t * actH + ((size_t)bt * H + j) * 32 + b];
-            float da = red_sum<2 * U>(red, u, b);
+            float da = red_sum<2 * V>(red, v, b);
             bw.DPA[t * actH + ((size_t)bt * H + j) * 32 + b] = da * (av > 0.f ? 1.f : av + 1.f);   // ELU'(pre) = a+1 for pre<=0
           }
-          bw.DH0[((size_t)bt * H + j) * 32 + b] = red_sum<2 * U>(red, U + u, b) + dhz0[(bt * U + u) * 32 + b];
+          bw.DH0[((size_t)bt * H + j) * 32 + b] = red_sum<2 * V>(red, V + v, b) + dhz0[(bt * U + u) * 32 + b];
         }
         __syncthreads();
       }
@@ -688,7 +696,8 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
     BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
     ScopedTimer tm("decoder_bwd", stream);
     const FilmDev none = {};
-    rc = g.U == 4 ? launch_bwd<4, false>(a, g, bg, w, bw, d, none, stream) : launch_bwd<8, false>(a, g, bg, w, bw, d, none, stream);
+    rc = g.U == 4 ? launch_bwd<4, false>(a, g, bg, w, bw, d, none, stream)
+       : g.U == 8 ? launch_bwd<8, false>(a, g, bg, w, bw, d, none, stream) : launch_bwd<16, false>(a, g, bg, w, bw, d, none, stream);
     if (rc) return rc;
   }
   ScopedTimer tm("decoder_wgrad", stream);
@@ -742,13 +751,13 @@ extern "C" int zeggs_decoder_window_bwd(const zeggs_decoder_fwd_args* ap, const 
 
 
 // ------------------------------------------------------------------ FiLM decoder (fp32 engine)
-// PBm[c][k][r] = Wm[k][c*U + r] (r < U, zero up to R1), behind the normal decoder's transposed slices
+// PBm[c][p][k][r] = Wm[k][c*U + p*V + r] (r < V, zero up to R1P = R1 / (U/V)), behind the normal decoder's transposed slices
 __global__ void pack_film_bwd_kernel(DecGeom g, int R1, const float* __restrict__ Wm, float* __restrict__ out) {
-  const int H = g.H, U = g.U;
+  const int H = g.H, U = g.U, V = pass_units(U), R1P = R1 / (U / V);
   const size_t total = (size_t)g.G * H * R1;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int r = i % R1, k = (i / R1) % H, c = i / ((size_t)R1 * H);
-    out[i] = r < U ? Wm[(size_t)k * H + c * U + r] : 0.f;
+    const int r = i % R1P, k = (i / R1P) % H, cp = i / ((size_t)R1P * H);   // cp = c * (U / V) + p
+    out[i] = r < V ? Wm[(size_t)k * H + cp * V + r] : 0.f;
   }
 }
 
@@ -848,7 +857,8 @@ extern "C" int zeggs_decoder_film_window_bwd(const zeggs_decoder_film_fwd_args* 
     const BwdGeom bg = make_bgeom(g);
     BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
     ScopedTimer tm("decoder_bwd", stream);
-    rc = g.U == 4 ? launch_bwd<4, true>(a, g, bg, w, bw, d, f, stream) : launch_bwd<8, true>(a, g, bg, w, bw, d, f, stream);
+    rc = g.U == 4 ? launch_bwd<4, true>(a, g, bg, w, bw, d, f, stream)
+       : g.U == 8 ? launch_bwd<8, true>(a, g, bg, w, bw, d, f, stream) : launch_bwd<16, true>(a, g, bg, w, bw, d, f, stream);
     if (rc) return rc;
   }
   ScopedTimer tm("decoder_wgrad", stream);

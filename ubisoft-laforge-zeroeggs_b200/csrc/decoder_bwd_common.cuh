@@ -5,7 +5,7 @@
 namespace zeggs {
 
 struct BwdGeom {
-  int R1;        // padded rows of the B1 tile (>= U, multiple of 8)
+  int R1;        // padded rows of the CTA's B1 tiles (>= U, multiple of 8; film_rows(pass_units(U)) per pass)
   int rpcb;      // x_pose-gradient rows per CTA (>= 9)
   int n4b;       // 16-row tiles per CTA for those rows
   size_t off2, off3a, off3b, off4, total;

@@ -61,12 +61,17 @@ int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs,
 int style_gru_rev_cell_fwd(int B, int H, const float* GIr, const float* bhh, float* hcat, cudaStream_t s);
 int style_gru_rev_cell_bwd(int B, int H, const float* GIr, const float* bhh, const float* dhcat, float* dGIr, float* dGHr, cudaStream_t s);
 
-// units per CTA: the grid G = H/U must fit one CTA per SM (132 on the H100 SXM)
+// units per CTA: the grid G = H/U must fit one CTA per SM (132 on the H100 SXM).  At U = 16 the fp32 recurrences run each stage as
+// two passes of 8 units (pass_units), so the register tiles and shared-memory stages stay those of U = 8.
 inline int pick_U(int H) {
   if (H % 4 == 0 && H / 4 <= 132) return 4;
   if (H % 8 == 0 && H / 8 <= 132) return 8;
+  if (H % 16 == 0 && H / 16 <= 132) return 16;
   return -1;
 }
+
+// units of one pass of the fp32 recurrences: a CTA's U units are U / pass_units(U) passes, each with its own contiguous weight slice
+__host__ __device__ constexpr int pass_units(int U) { return U < 8 ? U : 8; }
 
 // hidden sizes the tensor-core recurrence (engine 1: forward and BPTT kernels) covers; every tc size / pack / run entry point
 // applies this one rule (the BPTT kernel pairs 64-wide k-blocks, and below 384 nothing has been validated)
@@ -157,7 +162,7 @@ struct FilmDev {
 };
 
 // rows of the layer-2 FiLM tile (per-CTA units padded to the 8-row minimum of the skinny GEMM)
-__host__ __device__ inline int film_rows(int U) { return U < 8 ? 8 : U; }
+__host__ __device__ constexpr int film_rows(int U) { return U < 8 ? 8 : U; }
 
 // FiLM forward workspace: the normal decoder's carve-up followed by GB, E0, E2, C2; bytes = the whole workspace
 inline FilmDev make_film_ws(void* base, const DecWs& w, const DecGeom& g, int T, size_t* bytes) {

@@ -18,32 +18,35 @@
 namespace zeggs {
 
 // ------------------------------------------------------------------ weight packing
-// P1[c][k][r]  r in [0,4U): g=r/U (0: layer0, 1..3: W_ih0 gate g-1), unit j=c*U+r%U, k over pose cols
-// P2[c][k][r]  r in [0,6U): r<3U: W_ih0[g*H+j][k] (hidden cols), else W_hh0[g*H+j][k]
-// P3[c][k][r]  same with W_ih1 / W_hh1
+// CTA c's units are passes p of V = pass_units(U) units each (one pass below U = 16), unit j = c*U + p*V + r%V:
+// P1[c][p][k][r]  r in [0,4V): g=r/V (0: layer0, 1..3: W_ih0 gate g-1), k over pose cols
+// P2[c][p][k][r]  r in [0,6V): r<3V: W_ih0[g*H+j][k] (hidden cols), else W_hh0[g*H+j][k]
+// P3[c][p][k][r]  same with W_ih1 / W_hh1
 // P4[c][tile][k][16]  W2 rows c*rpc + tile*16 + r
 __global__ void pack_decoder_kernel(DecGeom g, const float* __restrict__ W0, const float* __restrict__ Wih0,
                                     const float* __restrict__ Whh0, const float* __restrict__ Wih1,
                                     const float* __restrict__ Whh1, const float* __restrict__ W2,
                                     float* __restrict__ out) {
   const size_t total = g.packed_floats();
-  const int H = g.H, U = g.U, A = g.A;
+  const int H = g.H, U = g.U, A = g.A, V = pass_units(U), NP = U / V;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     float v = 0.f;
     if (i < g.off_p2()) {
       size_t e = i;
-      int r = e % (4 * U); e /= (4 * U);
-      int k = e % K1P; int c = e / K1P;
-      int gi = r / U, j = c * U + r % U;
+      int r = e % (4 * V); e /= (4 * V);
+      int k = e % K1P; e /= K1P;
+      int p = e % NP, c = e / NP;
+      int gi = r / V, j = c * U + p * V + r % V;
       if (k < P_IN) v = (gi == 0) ? W0[(size_t)j * A + k] : Wih0[(size_t)((gi - 1) * H + j) * (A + H) + H + k];
     } else if (i < g.off_p4()) {
       const bool l1 = i >= g.off_p3();
       size_t e = i - (l1 ? g.off_p3() : g.off_p2());
-      int r = e % (6 * U); e /= (6 * U);
-      int k = e % H; int c = e / H;
-      const bool hh = r >= 3 * U;
-      int rr = hh ? r - 3 * U : r;
-      int gi = rr / U, j = c * U + rr % U;
+      int r = e % (6 * V); e /= (6 * V);
+      int k = e % H; e /= H;
+      int p = e % NP, c = e / NP;
+      const bool hh = r >= 3 * V;
+      int rr = hh ? r - 3 * V : r;
+      int gi = rr / V, j = c * U + p * V + rr % V;
       if (!l1) v = hh ? Whh0[(size_t)(gi * H + j) * H + k] : Wih0[(size_t)(gi * H + j) * (A + H) + k];
       else     v = hh ? Whh1[(size_t)(gi * H + j) * H + k] : Wih1[(size_t)(gi * H + j) * H + k];
     } else {
@@ -141,13 +144,15 @@ __global__ void __launch_bounds__(256) cond_precompute_kernel(zeggs_decoder_fwd_
 
 // ------------------------------------------------------------------ the persistent kernel
 // FILM: the FiLM decoder's step (modulated layer0, the extra layer2 stage, layer3 as the output layer; see FilmDev)
+// Stages 1-3 (and FiLM 3b) run once per pass of V units: the tiles are those of V units, the weight slices P1-P3 / P5 pass-major.
 template <int U, bool FILM>
 __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, DecWs w, FilmDev f) {
   extern __shared__ __align__(16) float smem[];
-  constexpr int RT1 = U, RT2 = (6 * U) / 4;
+  constexpr int V = pass_units(U), NP = U / V;
+  constexpr int RT1 = V, RT2 = (6 * V) / 4;
   float* stage = smem;                                  // 8 warps x 2 x STG_MAX
-  float* red = smem + 8 * 2 * SkinnyCfg<RT2>::STG;      // [8][6U][32]
-  float* gi0p = red + 8 * 6 * U * 32;                   // [nbt][3][U][32]
+  float* red = smem + 8 * 2 * SkinnyCfg<RT2>::STG;      // [8][6V][32]
+  float* gi0p = red + 8 * 6 * V * 32;                   // [nbt][3][U][32]
   float* rootv = gi0p + g.nbt * 3 * U * 32;             // [6][32]
   const int c = blockIdx.x, tid = threadIdx.x, warp = tid >> 5;
   const int H = a.H, T = a.T, nbt = g.nbt;
@@ -158,24 +163,25 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
   const float* P2 = a.packed + g.off_p2() + (size_t)c * H * 6 * U;
   const float* P3 = a.packed + g.off_p3() + (size_t)c * H * 6 * U;
   const float* P4 = a.packed + g.off_p4() + (size_t)c * g.n4t * H * 16;
-  constexpr int RTM = (U < 8 ? 8 : U) / 4;       // FiLM layer2 tile (film_rows(U) rows)
-  const float* P5 = a.packed + g.packed_floats() + (size_t)c * H * 4 * RTM;
+  constexpr int RTM = film_rows(V) / 4;          // FiLM layer2 tile (film_rows(V) rows per pass)
+  const float* P5 = a.packed + g.packed_floats() + (size_t)c * NP * H * 4 * RTM;
   const size_t actH = (size_t)nbt * H * 32;      // floats per time slot of an [nbt][H][32] buffer
   const size_t actX = (size_t)nbt * K1P * 32;
 
   for (int t = 1; t < T; ++t) {
     const int ts = w.save ? t : (t & 1), tp = w.save ? t - 1 : ((t - 1) & 1), tn = w.save ? t + 1 : ((t + 1) & 1);
     // ------------------------------------------------------------ stage 1
-    for (int bt = 0; bt < nbt; ++bt) {
+    for (int q = 0; q < nbt * NP; ++q) {
+      const int bt = q / NP, p = q % NP;
       float acc[RT1][4];
       const float* x = w.XP + ts * actX + (size_t)bt * K1P * 32;
-      skinny_gemm<RT1, false>(acc, P1, x, x, K1P / 16, wstage);
+      skinny_gemm<RT1, false>(acc, P1 + (size_t)p * K1P * 4 * V, x, x, K1P / 16, wstage);
       reduce_store<RT1>(acc, red);
       __syncthreads();
-      for (int idx = tid; idx < U * 32; idx += 256) {
-        const int u = idx >> 5, b = idx & 31, j = c * U + u;
+      for (int idx = tid; idx < V * 32; idx += 256) {
+        const int u = p * V + (idx >> 5), b = idx & 31, j = c * U + u;
         const float* S = w.S01 + (((size_t)t * nbt + bt) * 4 * H) * 32;
-        float pre = red_sum<4 * U>(red, u, b) + S[(size_t)j * 32 + b];
+        float pre = red_sum<4 * V>(red, idx >> 5, b) + S[(size_t)j * 32 + b];
         if constexpr (FILM) {
           const int bgl = bt * 32 + b;
           const float* gb = f.GB + ((size_t)bgl * T + t) * 4 * H;
@@ -187,27 +193,28 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
         }
 #pragma unroll
         for (int gi = 0; gi < 3; ++gi)
-          gi0p[((bt * 3 + gi) * U + u) * 32 + b] = red_sum<4 * U>(red, (1 + gi) * U + u, b) + S[(size_t)(H + gi * H + j) * 32 + b];
+          gi0p[((bt * 3 + gi) * U + u) * 32 + b] = red_sum<4 * V>(red, (1 + gi) * V + (idx >> 5), b) + S[(size_t)(H + gi * H + j) * 32 + b];
       }
       __syncthreads();
     }
     if (!grid_sync(gb)) return;
     // ------------------------------------------------------------ stage 2 (GRU layer 0)
-    for (int bt = 0; bt < nbt; ++bt) {
+    for (int q = 0; q < nbt * NP; ++q) {
+      const int bt = q / NP, p = q % NP;
       float acc[RT2][4];
       const float* xa = w.A + ts * actH + (size_t)bt * H * 32;
       const float* xb = w.H0 + tp * actH + (size_t)bt * H * 32;
-      skinny_gemm<RT2, true>(acc, P2, xa, xb, H / 16, wstage);
+      skinny_gemm<RT2, true>(acc, P2 + (size_t)p * H * 6 * V, xa, xb, H / 16, wstage);
       reduce_store<RT2>(acc, red);
       __syncthreads();
-      for (int idx = tid; idx < U * 32; idx += 256) {
-        const int u = idx >> 5, b = idx & 31, j = c * U + u;
-        float gir = red_sum<6 * U>(red, 0 * U + u, b) + gi0p[((bt * 3 + 0) * U + u) * 32 + b];
-        float giz = red_sum<6 * U>(red, 1 * U + u, b) + gi0p[((bt * 3 + 1) * U + u) * 32 + b];
-        float gin = red_sum<6 * U>(red, 2 * U + u, b) + gi0p[((bt * 3 + 2) * U + u) * 32 + b];
-        float ghr = red_sum<6 * U>(red, 3 * U + u, b) + a.b_hh0[0 * H + j];
-        float ghz = red_sum<6 * U>(red, 4 * U + u, b) + a.b_hh0[1 * H + j];
-        float ghn = red_sum<6 * U>(red, 5 * U + u, b) + a.b_hh0[2 * H + j];
+      for (int idx = tid; idx < V * 32; idx += 256) {
+        const int u = p * V + (idx >> 5), v = idx >> 5, b = idx & 31, j = c * U + u;
+        float gir = red_sum<6 * V>(red, 0 * V + v, b) + gi0p[((bt * 3 + 0) * U + u) * 32 + b];
+        float giz = red_sum<6 * V>(red, 1 * V + v, b) + gi0p[((bt * 3 + 1) * U + u) * 32 + b];
+        float gin = red_sum<6 * V>(red, 2 * V + v, b) + gi0p[((bt * 3 + 2) * U + u) * 32 + b];
+        float ghr = red_sum<6 * V>(red, 3 * V + v, b) + a.b_hh0[0 * H + j];
+        float ghz = red_sum<6 * V>(red, 4 * V + v, b) + a.b_hh0[1 * H + j];
+        float ghn = red_sum<6 * V>(red, 5 * V + v, b) + a.b_hh0[2 * H + j];
         float r = sigmoid_f(gir + ghr), z = sigmoid_f(giz + ghz);
         float n = tanhf(gin + r * ghn);
         float hp = ld_cg(xb + (size_t)j * 32 + b);
@@ -223,21 +230,22 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
     }
     if (!grid_sync(gb)) return;
     // ------------------------------------------------------------ stage 3 (GRU layer 1)
-    for (int bt = 0; bt < nbt; ++bt) {
+    for (int q = 0; q < nbt * NP; ++q) {
+      const int bt = q / NP, p = q % NP;
       float acc[RT2][4];
       const float* xa = w.H0 + ts * actH + (size_t)bt * H * 32;
       const float* xb = w.H1 + tp * actH + (size_t)bt * H * 32;
-      skinny_gemm<RT2, true>(acc, P3, xa, xb, H / 16, wstage);
+      skinny_gemm<RT2, true>(acc, P3 + (size_t)p * H * 6 * V, xa, xb, H / 16, wstage);
       reduce_store<RT2>(acc, red);
       __syncthreads();
-      for (int idx = tid; idx < U * 32; idx += 256) {
-        const int u = idx >> 5, b = idx & 31, j = c * U + u;
-        float gir = red_sum<6 * U>(red, 0 * U + u, b) + a.b_ih1[0 * H + j];
-        float giz = red_sum<6 * U>(red, 1 * U + u, b) + a.b_ih1[1 * H + j];
-        float gin = red_sum<6 * U>(red, 2 * U + u, b) + a.b_ih1[2 * H + j];
-        float ghr = red_sum<6 * U>(red, 3 * U + u, b) + a.b_hh1[0 * H + j];
-        float ghz = red_sum<6 * U>(red, 4 * U + u, b) + a.b_hh1[1 * H + j];
-        float ghn = red_sum<6 * U>(red, 5 * U + u, b) + a.b_hh1[2 * H + j];
+      for (int idx = tid; idx < V * 32; idx += 256) {
+        const int u = p * V + (idx >> 5), v = idx >> 5, b = idx & 31, j = c * U + u;
+        float gir = red_sum<6 * V>(red, 0 * V + v, b) + a.b_ih1[0 * H + j];
+        float giz = red_sum<6 * V>(red, 1 * V + v, b) + a.b_ih1[1 * H + j];
+        float gin = red_sum<6 * V>(red, 2 * V + v, b) + a.b_ih1[2 * H + j];
+        float ghr = red_sum<6 * V>(red, 3 * V + v, b) + a.b_hh1[0 * H + j];
+        float ghz = red_sum<6 * V>(red, 4 * V + v, b) + a.b_hh1[1 * H + j];
+        float ghn = red_sum<6 * V>(red, 5 * V + v, b) + a.b_hh1[2 * H + j];
         float r = sigmoid_f(gir + ghr), z = sigmoid_f(giz + ghz);
         float n = tanhf(gin + r * ghn);
         float hp = ld_cg(xb + (size_t)j * 32 + b);
@@ -254,15 +262,16 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
     if (!grid_sync(gb)) return;
     if constexpr (FILM) {
       // ---------------------------------------------------------- stage 3b (FiLM layer2: c = ELU(Wm h1 + bm) * g[H:] + be[H:])
-      for (int bt = 0; bt < nbt; ++bt) {
+      for (int q = 0; q < nbt * NP; ++q) {
+        const int bt = q / NP, p = q % NP;
         float acc[RTM][4];
         const float* x = w.H1 + ts * actH + (size_t)bt * H * 32;
-        skinny_gemm<RTM, false>(acc, P5, x, x, H / 16, wstage);
+        skinny_gemm<RTM, false>(acc, P5 + (size_t)p * H * 4 * RTM, x, x, H / 16, wstage);
         reduce_store<RTM>(acc, red);
         __syncthreads();
-        for (int idx = tid; idx < U * 32; idx += 256) {
-          const int u = idx >> 5, b = idx & 31, j = c * U + u, bgl = bt * 32 + b;
-          const float e = elu_f(red_sum<4 * RTM>(red, u, b) + f.bm[j]);
+        for (int idx = tid; idx < V * 32; idx += 256) {
+          const int b = idx & 31, j = c * U + p * V + (idx >> 5), bgl = bt * 32 + b;
+          const float e = elu_f(red_sum<4 * RTM>(red, idx >> 5, b) + f.bm[j]);
           const float* gbr = f.GB + ((size_t)bgl * T + t) * 4 * H;
           f.C2[ts * actH + ((size_t)bt * H + j) * 32 + b] = bgl < a.B ? e * (1.f + gbr[H + j]) + gbr[3 * H + j] : e;   // modules.py:224-225
           if (w.save) f.E2[ts * actH + ((size_t)bt * H + j) * 32 + b] = e;
@@ -328,17 +337,18 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
 // dynamic shared memory per CTA of the fp32 recurrence: it grows with the 32-sample batch tiles, which bounds the batch of one call
 template <int U>
 static size_t fwd_smem_bytes(int nbt) {
-  constexpr int RT2 = (6 * U) / 4;
-  return (size_t)(8 * 2 * SkinnyCfg<RT2>::STG + 8 * 6 * U * 32 + nbt * 3 * U * 32 + 6 * 32) * sizeof(float);
+  constexpr int V = pass_units(U), RT2 = (6 * V) / 4;
+  return (size_t)(8 * 2 * SkinnyCfg<RT2>::STG + 8 * 6 * V * 32 + nbt * 3 * U * 32 + 6 * 32) * sizeof(float);
 }
 
 static int check_fwd_args(const zeggs_decoder_fwd_args* a) {
   ZCHECK_ARG(a != nullptr, "decoder: null args");
   ZCHECK_ARG(a->B >= 1 && a->T >= 1, "decoder: bad B=%d T=%d", a->B, a->T);
-  ZCHECK_ARG(a->H % 16 == 0 && pick_U(a->H) > 0, "decoder: hidden size %d unsupported (need H%%16==0, H<=1056)", a->H);
+  ZCHECK_ARG(a->H % 16 == 0 && pick_U(a->H) > 0, "decoder: hidden size %d unsupported (need H%%16==0, H<=2112)", a->H);
   ZCHECK_ARG(a->S >= 1 && a->Z >= 1 && a->S + a->Z <= 256, "decoder: bad S=%d Z=%d", a->S, a->Z);
   if (a->engine != 1) {
-    size_t (*smem_of)(int) = pick_U(a->H) == 4 ? fwd_smem_bytes<4> : fwd_smem_bytes<8>;
+    const int U = pick_U(a->H);
+    size_t (*smem_of)(int) = U == 4 ? fwd_smem_bytes<4> : U == 8 ? fwd_smem_bytes<8> : fwd_smem_bytes<16>;
     const int nbt = ceil_div(a->B, 32);
     int dev = 0, cap = 0;
     ZCHECK_CUDA(cudaGetDevice(&dev));
@@ -399,6 +409,7 @@ static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& 
   ZCHECK_LAUNCH();
   ScopedTimer tm("decoder_fwd", stream);
   const FilmDev none = {};
+  if (g.U == 16) return launch_fwd<16, false>(a, g, w, none, stream);
   return g.U == 4 ? launch_fwd<4, false>(a, g, w, none, stream) : launch_fwd<8, false>(a, g, w, none, stream);
 }
 
@@ -439,13 +450,13 @@ extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* 
 }
 
 // ------------------------------------------------------------------ FiLM decoder (fp32 engine)
-// P5[c][k][r] = Wm[c*U + r][k] (r < U; rows up to film_rows(U) are zero), behind the normal decoder's slices
+// P5[c][p][k][r] = Wm[c*U + p*V + r][k] (r < V; rows up to film_rows(V) are zero), behind the normal decoder's slices
 __global__ void pack_film_kernel(DecGeom g, const float* __restrict__ Wm, float* __restrict__ out) {
-  const int H = g.H, U = g.U, R = film_rows(g.U);
-  const size_t total = (size_t)g.G * H * R;
+  const int H = g.H, U = g.U, V = pass_units(U), R = film_rows(V);
+  const size_t total = (size_t)g.G * (U / V) * H * R;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int r = i % R, k = (i / R) % H, c = i / ((size_t)R * H);
-    out[i] = r < U ? Wm[(size_t)(c * U + r) * H + k] : 0.f;
+    const int r = i % R, k = (i / R) % H, cp = i / ((size_t)R * H);   // cp = c * (U / V) + p
+    out[i] = r < V ? Wm[(size_t)(cp * V + r) * H + k] : 0.f;
   }
 }
 
@@ -514,6 +525,7 @@ extern "C" int zeggs_decoder_film_window_fwd(const zeggs_decoder_film_fwd_args* 
   count_launch();
   ZCHECK_LAUNCH();
   ScopedTimer tm("decoder_fwd", stream);
+  if (g.U == 16) return launch_fwd<16, true>(a, g, w, f, stream);
   return g.U == 4 ? launch_fwd<4, true>(a, g, w, f, stream) : launch_fwd<8, true>(a, g, w, f, stream);
 }
 
