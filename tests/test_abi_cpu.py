@@ -1,5 +1,6 @@
 """CPU-only checks: the C-ABI library builds (nvcc cross-compile), loads and exports every symbol
 include/zeggs_b200.h declares; host-side table construction matches the oracle; no compute calls."""
+import json
 import os
 import re
 
@@ -48,6 +49,35 @@ def test_mel_frame_count_rule(built):
         assert l.zeggs_mel_num_frames(ns, 800, hop) == mel_oracle.num_frames(ns, 800, hop)
 
 
+def _size_table(l):
+    """Every *_bytes query of the header over a small grid of shapes (zeros included), keyed by query name: the layouts of the
+    workspaces and packed weights are part of the ABI, and phase 2 of the decoder backward relies on the same carve-up as phase 1."""
+    Hs, Bs, Ts, Zs, S = (16, 64, 384, 1024, 1056, 1072, 2112, 2128), (1, 32, 33), (1, 2, 256), (9, 64), 64
+    q = lambda name, shapes: [int(getattr(l, "zeggs_" + name)(*s)) for s in shapes]
+    packed = [(H, S, Z) for H in Hs for Z in Zs]
+    ws = [(B, T, H, S, Z) for H in Hs for B in Bs for T in Ts for Z in Zs]
+    ws_save = [s + (save,) for s in ws for save in (0, 1)]
+    t = {name: q(name, packed) for name in ("decoder_packed_bytes", "decoder_packed_tc_bytes", "decoder_tc_workspace_bytes",
+                                            "decoder_packed_bwd_bytes", "decoder_packed_bwd_tc_bytes", "decoder_bwd_tc_workspace_bytes",
+                                            "decoder_packed_film_bytes", "decoder_packed_bwd_film_bytes")}
+    t.update({name: q(name, ws_save) for name in ("decoder_workspace_bytes", "decoder_film_workspace_bytes")})
+    t.update({name: q(name, ws) for name in ("decoder_bwd_workspace_bytes", "decoder_film_bwd_workspace_bytes")})
+    t["decoder_step_workspace_bytes"] = q("decoder_step_workspace_bytes", [(B, H, S, Z) for H in Hs for B in Bs for Z in Zs] + [(0, 64, 64, 64)])
+    t["speech_enc_workspace_bytes"] = q("speech_enc_workspace_bytes", [(1, 1, 80, 64, 64), (32, 34, 81, 128, 64), (64, 256, 80, 256, 128),
+                                                                       (0, 34, 81, 128, 64)])
+    t["style_enc_workspace_bytes"] = q("style_enc_workspace_bytes", [(1, 1, 1134, 256, 128, 2), (32, 256, 1134, 256, 128, 2),
+                                                                     (7, 33, 1131, 64, 64, 4), (7, 33, 1131, 64, 63, 4)])
+    t["style_enc_gru_workspace_bytes"] = q("style_enc_gru_workspace_bytes", [(1, 1, 1134, 64, 64, 0), (32, 256, 1134, 1056, 128, 1),
+                                                                             (1216, 17, 1134, 1056, 128, 1), (33, 2, 10, 528, 9, 0),
+                                                                             (33, 2, 10, 528, 9, 1), (1, 1, 1134, 532, 64, 0)])
+    t["loss_workspace_bytes"] = q("loss_workspace_bytes", [(1, 1), (32, 256), (33, 2), (0, 5)])
+    t["loudness_workspace_bytes"] = q("loudness_workspace_bytes", [(1, 1), (4, 100), (32, 1000), (0, 10)])
+    t["anim_features_workspace_bytes"] = q("anim_features_workspace_bytes", [(1, 75), (256, 75), (1000, 3), (0, 75)])
+    t["spline_resample_workspace_bytes"] = q("spline_resample_workspace_bytes", [(1, 1), (1000, 1131), (10 ** 6, 3), (0, 3)])
+    t["masked_moments_workspace_bytes"] = q("masked_moments_workspace_bytes", [(1, 1), (1000, 1131), (10 ** 6, 75), (0, 75)])
+    return t
+
+
 def test_workspace_and_pack_sizes(built):
     l = built.lib()
     assert l.zeggs_decoder_packed_bytes(1024, 64, 64) > 4 * (1024 * 1134 * 4 + 12 * 1024 * 1024)
@@ -55,6 +85,13 @@ def test_workspace_and_pack_sizes(built):
     a = l.zeggs_decoder_workspace_bytes(32, 256, 1024, 64, 64, 1)
     b = l.zeggs_decoder_workspace_bytes(32, 256, 1024, 64, 64, 0)
     assert a > b > 0
+    # the exact sizes: any change to a workspace or pack layout shows up here
+    with open(os.path.join(ROOT, "tests", "golden", "workspace_sizes.json")) as f:
+        want = json.load(f)
+    got = _size_table(l)
+    hdr = open(os.path.join(ROOT, "include", "zeggs_b200.h")).read()
+    assert set(got) == {n[len("zeggs_"):] for n in re.findall(r"\b(zeggs_[a-z0-9_]+_bytes)\s*\(", hdr)}
+    assert got == want
 
 
 def test_style_gru_refuses_batches_its_backward_cannot_hold(built):

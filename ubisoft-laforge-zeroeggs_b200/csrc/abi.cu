@@ -1,11 +1,12 @@
-// Error plumbing, launch counter and version for the C ABI (include/zeggs_b200.h).
+// Error plumbing, launch counter, per-device launch limits and version for the C ABI (include/zeggs_b200.h).
 #include <cstring>
 #include <stdarg.h>
 #include <atomic>
+#include <map>
 #include <mutex>
+#include <tuple>
 #include <vector>
-#include "common.cuh"
-#include "../../include/zeggs_b200.h"
+#include "library.cuh"
 
 namespace zeggs {
 static thread_local char g_err[1024] = "";
@@ -19,6 +20,70 @@ void set_error(const char* fmt, ...) {
 }
 const char* get_error() { return g_err; }
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+
+// ---------------------------------------------------------------- launch limits, per device ordinal
+int device_limits(DeviceLimits* lim) {
+  static std::mutex mu;
+  static std::map<int, DeviceLimits> known;
+  int dev = 0;
+  ZCHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = known.find(dev);
+  if (it == known.end()) {
+    int sms = 0, smem = 0;
+    ZCHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    ZCHECK_CUDA(cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    it = known.emplace(dev, DeviceLimits{sms, (size_t)smem}).first;
+  }
+  *lim = it->second;
+  return ZEGGS_OK;
+}
+
+int set_max_dynamic_smem(const void* kernel, size_t smem) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limit;   // (kernel, device) -> the limit set there
+  int dev = 0;
+  ZCHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(mu);
+  size_t& cur = limit[{kernel, dev}];
+  if (smem > cur) {
+    ZCHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cur = smem;
+  }
+  return ZEGGS_OK;
+}
+
+int persistent_capacity(const void* kernel, int block, size_t smem, int cluster, int* ctas) {
+  static std::mutex mu;
+  static std::map<std::tuple<const void*, int, size_t>, int> known;   // (kernel, device, smem) -> resident CTAs
+  int dev = 0;
+  ZCHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = known.find({kernel, dev, smem});
+  if (it == known.end()) {
+    int rc = set_max_dynamic_smem(kernel, smem);
+    if (rc) return rc;
+    int n = 0;
+    if (cluster == 1) {
+      DeviceLimits lim;
+      if ((rc = device_limits(&lim))) return rc;
+      ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, block, smem));
+      n *= lim.sms;
+    } else {
+      cudaLaunchAttribute attr;
+      attr.id = cudaLaunchAttributeClusterDimension;
+      attr.val.clusterDim.x = cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = dim3(cluster); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem;
+      cfg.attrs = &attr; cfg.numAttrs = 1;
+      ZCHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kernel, &cfg));
+      n *= cluster;
+    }
+    it = known.emplace(std::make_tuple(kernel, dev, smem), n).first;
+  }
+  *ctas = it->second;
+  return ZEGGS_OK;
+}
 }  // namespace zeggs
 
 // ---------------------------------------------------------------- live kernel timer (bench.py's roofline leg)

@@ -484,14 +484,14 @@ __global__ void __launch_bounds__(256) dy_combine_kernel(zeggs_decoder_fwd_args 
 
 // ------------------------------------------------------------------ host
 extern "C" size_t zeggs_decoder_packed_bwd_bytes(int H, int S, int Z) {
-  if (H % 16 != 0 || pick_U(H) <= 0) return 0;
+  if (!fp32_hidden_ok(H)) return 0;
   DecGeom g = make_geom(1, H, S, Z);
   return make_bgeom(g).total * sizeof(float);
 }
 
 extern "C" int zeggs_decoder_pack_weights_bwd(const zeggs_decoder_fwd_args* a, float* packed, void* stream_) {
   CtxScope ctx_scope(a ? a->ctx : nullptr);
-  ZCHECK_ARG(a && packed && a->H % 16 == 0 && pick_U(a->H) > 0, "decoder bwd pack: bad arguments");
+  ZCHECK_ARG(a && packed && fp32_hidden_ok(a->H), "decoder bwd pack: bad arguments");
   DecGeom g = make_geom(a->B, a->H, a->S, a->Z);
   BwdGeom bg = make_bgeom(g);
   pack_decoder_bwd_kernel<<<592, 256, 0, (cudaStream_t)stream_>>>(g, bg, a->W0, a->W_ih0, a->W_hh0, a->W_ih1, a->W_hh1, a->W2, packed);
@@ -501,34 +501,31 @@ extern "C" int zeggs_decoder_pack_weights_bwd(const zeggs_decoder_fwd_args* a, f
 }
 
 extern "C" size_t zeggs_decoder_bwd_workspace_bytes(int B, int T, int H, int S, int Z) {
-  if (H % 16 != 0 || pick_U(H) <= 0 || B < 1 || T < 1) return 0;
+  if (!fp32_hidden_ok(H) || B < 1 || T < 1) return 0;
   DecGeom g = make_geom(B, H, S, Z);
   return make_bws(nullptr, g, T).bytes;
+}
+
+// dynamic shared memory per CTA of the BPTT recurrence: it grows with the 32-sample batch tiles, which bounds the batch of one call
+static size_t bwd_smem_bytes(const DecGeom& g, const BwdGeom& bg, int nbt) {
+  return (size_t)(8 * 2 * SkinnyCfg<4>::STG + 8 * 16 * 32 + 2 * nbt * g.U * 32 + nbt * bg.n4b * 16 * 32 + nbt * 9 * 32 + nbt * 7 * 32) *
+         sizeof(float);
+}
+
+// the fp32 backward, normal and FiLM, refuses a batch its shared memory cannot hold before it enqueues anything
+static int check_bwd_batch(const DecGeom& g, const BwdGeom& bg) {
+  DeviceLimits lim;
+  RC(device_limits(&lim));
+  auto smem_of = [&](int nbt) { return bwd_smem_bytes(g, bg, nbt); };
+  ZCHECK_ARG(smem_of(g.nbt) <= lim.smem_optin, "decoder bwd: batch %d needs %zu bytes of shared memory per CTA at hidden size %d (%zu "
+             "available): at most %d samples per call", g.B, smem_of(g.nbt), g.H, lim.smem_optin, 32 * max_batch_tiles(smem_of, lim.smem_optin));
+  return ZEGGS_OK;
 }
 
 template <int U, bool FILM>
 static int launch_bwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdGeom& bg, const DecWs& w, const BwdWs& bw,
                       const BwdArgsDev& d, const FilmDev& f, cudaStream_t stream) {
-  // dynamic shared memory per CTA: it grows with the 32-sample batch tiles, which bounds the batch of one call
-  auto smem_of = [&](int nbt) {
-    return (size_t)(8 * 2 * SkinnyCfg<4>::STG + 8 * 16 * 32 + 2 * nbt * U * 32 + nbt * bg.n4b * 16 * 32 + nbt * 9 * 32 + nbt * 7 * 32) * sizeof(float);
-  };
-  const size_t smem = smem_of(g.nbt);
-  int dev = 0, nsm = 0, occ = 0, cap = 0;
-  ZCHECK_CUDA(cudaGetDevice(&dev));
-  ZCHECK_CUDA(cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  int max_nbt = g.nbt;
-  while (max_nbt > 0 && smem_of(max_nbt) > (size_t)cap) --max_nbt;
-  ZCHECK_ARG(smem <= (size_t)cap, "decoder bwd: batch %d needs %zu bytes of shared memory per CTA at hidden size %d (%d available): at most "
-             "%d samples per call", g.B, smem, g.H, cap, 32 * max_nbt);
-  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_bwd_kernel<U, FILM>, 256, smem));
-  ZCHECK_ARG(occ * nsm >= g.G, "decoder bwd: cooperative grid of %d CTAs does not fit", g.G);
-  void* args[] = {(void*)&a, (void*)&g, (void*)&bg, (void*)&w, (void*)&bw, (void*)&d, (void*)&f};
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_bwd_kernel<U, FILM>, dim3(g.G), dim3(256), args, smem, stream));
-  count_launch();
-  return ZEGGS_OK;
+  return launch_persistent(decoder_bwd_kernel<U, FILM>, g.G, 256, bwd_smem_bytes(g, bg, g.nbt), 1, stream, a, g, bg, w, bw, d, f);
 }
 
 static int wgrad(const float* GA, long long gaT, long long gaBT, int N, const float* XB, long long xbT, long long xbBT, int K,
@@ -557,17 +554,10 @@ WgradHists wgrad_hists(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_
   hs.slots = a.T * nbt;
   hs.nbt = nbt;
   hs.ld = (size_t)hs.slots * 32;
-  char* base = scratch_base();
-  size_t off = 0;
-  auto take = [&](int rows) {
-    __nv_bfloat16* p = base ? (__nv_bfloat16*)(base + off) : nullptr;
-    off += (size_t)rows * hs.ld * 2;
-    return p;
-  };
-  for (auto& h : hs.h) h.hi = take(h.rows);
-  if (want_lo) for (auto& h : hs.h) h.lo = take(h.rows);
-  hs.bytes = off;
-  hs.end = base ? base + off : nullptr;
+  Arena sc{scratch_base(), 0, 1};   // rows of (ld * 2) bytes: no rounding between the copies, they stack into one operand
+  for (auto& h : hs.h) h.hi = (__nv_bfloat16*)sc.bytes((size_t)h.rows * hs.ld * 2);
+  if (want_lo) for (auto& h : hs.h) h.lo = (__nv_bfloat16*)sc.bytes((size_t)h.rows * hs.ld * 2);
+  hs.bytes = sc.off;
   return hs;
 }
 
@@ -579,19 +569,18 @@ int split_hist(const WgradHists& hs, int i, cudaStream_t stream) {
 }
 
 int wgrad_gemms(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const WgradHists& hs, bool want_lo,
-                char* tail, cudaStream_t stream) {
+                Arena tail, cudaStream_t stream) {
   const int H = a.H, A = g.A, C = a.S + a.Z;
   const int cur = g.nbt * 32;                       // column offset of slot t = 1
   const int Kc = (a.T - 1) * g.nbt * 32;
-  char* const end = scratch_base() + scratch_bytes();
-  char* ws_p = (char*)(((uintptr_t)tail + 255) & ~(uintptr_t)255);
   // the histories may end within 255 bytes of the scratch end: the aligned tail then lies past it and there is no split-K room
-  const size_t ws_bytes = ws_p < end ? (size_t)(end - ws_p) : 0;
+  float* const ws = (float*)tail.align(256).here();
+  const size_t ws_bytes = tail.rest(scratch_bytes());
   auto G = [&](int ga, int ga_off, int N, int xb, int xb_off, int K, float* dW, int ldw) {
     const WgradHist &x = hs.h[ga], &y = hs.h[xb];
     return tc_gemm_launch(N, K, Kc, x.hi + ga_off, want_lo ? x.lo + ga_off : nullptr, (int)hs.ld,
                           y.hi + xb_off, want_lo ? y.lo + xb_off : nullptr, (int)hs.ld, nullptr, dW, ldw, 0, 0, stream,
-                          (float*)ws_p, ws_bytes);
+                          ws, ws_bytes);
   };
   int rc;
   if ((rc = G(HDY, cur, P_OUT, HH1, cur, H, b.dW2, H))) return rc;
@@ -688,11 +677,12 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
   ZCHECK_ARG(b.packed_bwd, "decoder bwd: packed_bwd missing");
   if (b.phase == 2) return ZEGGS_OK;
   const int T = a.T, nbt = g.nbt;
+  const BwdGeom bg = make_bgeom(g);
   int rc;
+  RC(check_bwd_batch(g, bg));
   ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
   ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
   {
-    const BwdGeom bg = make_bgeom(g);
     BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
     ScopedTimer tm("decoder_bwd", stream);
     const FilmDev none = {};
@@ -708,7 +698,7 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
   const WgradHists hs = wgrad_hists(a, b, g, w, bw, want_lo);
   if (gemm_mode() == 1 && scratch_base() != nullptr && hs.bytes <= scratch_bytes()) {
     for (int i = 0; i < NHIST; ++i) if ((rc = split_hist(hs, i, stream))) return rc;
-    if ((rc = wgrad_gemms(a, b, g, hs, want_lo, hs.end, stream))) return rc;
+    if ((rc = wgrad_gemms(a, b, g, hs, want_lo, Arena{scratch_base(), hs.bytes, 1}, stream))) return rc;
   } else {
     if ((rc = wgrad_simt(a, b, g, w, bw, w.H1, stream))) return rc;
   }
@@ -781,14 +771,14 @@ __global__ void film_style0_kernel(int B, int T, int Z, const float* __restrict_
 static size_t film_bwd_extra_floats(const DecGeom& g) { return (size_t)g.G * g.H * make_bgeom(g).R1; }
 
 extern "C" size_t zeggs_decoder_packed_bwd_film_bytes(int H, int S, int Z) {
-  if (H % 16 != 0 || pick_U(H) <= 0) return 0;
+  if (!fp32_hidden_ok(H)) return 0;
   DecGeom g = make_film_geom(1, H, S, Z);
   return (make_bgeom(g).total + film_bwd_extra_floats(g)) * sizeof(float);
 }
 
 extern "C" int zeggs_decoder_pack_weights_bwd_film(const zeggs_decoder_film_fwd_args* f, float* packed, void* stream_) {
   CtxScope ctx_scope(f ? f->dec.ctx : nullptr);
-  ZCHECK_ARG(f && packed && f->Wm && f->dec.H % 16 == 0 && pick_U(f->dec.H) > 0, "film decoder bwd pack: bad arguments");
+  ZCHECK_ARG(f && packed && f->Wm && fp32_hidden_ok(f->dec.H), "film decoder bwd pack: bad arguments");
   const zeggs_decoder_fwd_args& a = f->dec;
   DecGeom g = make_film_geom(a.B, a.H, a.S, a.Z);
   BwdGeom bg = make_bgeom(g);
@@ -803,19 +793,14 @@ extern "C" int zeggs_decoder_pack_weights_bwd_film(const zeggs_decoder_film_fwd_
 
 // backward workspace: the normal decoder's carve-up followed by DGB [B*T][4H] and DP2 [T][nbt][H][32]
 static size_t film_bwd_ws(void* base, const DecGeom& g, int T, FilmDev& f) {
-  size_t off = make_bws(nullptr, g, T).bytes;
-  auto take = [&](size_t nfloats) {
-    float* p = base ? (float*)((char*)base + off) : nullptr;
-    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
-    return p;
-  };
-  f.DGB = take((size_t)g.B * T * 4 * g.H);
-  f.DP2 = take((size_t)T * g.nbt * g.H * 32);
-  return off;
+  Arena a{(char*)base, make_bws(nullptr, g, T).bytes};
+  f.DGB = a.take((size_t)g.B * T * 4 * g.H);
+  f.DP2 = a.take((size_t)T * g.nbt * g.H * 32);
+  return a.off;
 }
 
 extern "C" size_t zeggs_decoder_film_bwd_workspace_bytes(int B, int T, int H, int S, int Z) {
-  if (H % 16 != 0 || pick_U(H) <= 0 || B < 1 || T < 1) return 0;
+  if (!fp32_hidden_ok(H) || B < 1 || T < 1) return 0;
   FilmDev f = {};
   return film_bwd_ws(nullptr, make_film_geom(B, H, S, Z), T, f);
 }
@@ -849,12 +834,13 @@ extern "C" int zeggs_decoder_film_window_bwd(const zeggs_decoder_film_fwd_args* 
   ZCHECK_ARG(a.workspace_bytes >= fwd_bytes, "film decoder bwd: forward workspace too small (%zu < %zu)", a.workspace_bytes, fwd_bytes);
   ZCHECK_ARG(b.workspace && b.workspace_bytes >= need, "film decoder bwd: workspace too small (%zu < %zu)", b.workspace_bytes, need);
   const int nbt = g.nbt, BT = a.B * T;
+  const BwdGeom bg = make_bgeom(g);
   int rc;
+  RC(check_bwd_batch(g, bg));
   ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
   ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
   ZCHECK_CUDA(cudaMemsetAsync(f.DGB, 0, (size_t)BT * 4 * H * sizeof(float), stream));
   {
-    const BwdGeom bg = make_bgeom(g);
     BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
     ScopedTimer tm("decoder_bwd", stream);
     rc = g.U == 4 ? launch_bwd<4, true>(a, g, bg, w, bw, d, f, stream)

@@ -40,25 +40,20 @@ struct BwdWs {
 
 inline BwdWs make_bws(void* base, const DecGeom& g, int T) {
   BwdWs w;
-  size_t off = 0;
-  auto take = [&](size_t nfloats) {
-    float* p = base ? (float*)((char*)base + off) : nullptr;
-    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
-    return p;
-  };
+  Arena a{(char*)base};
   const size_t S = (size_t)T * g.nbt;
   const int C = g.S + g.Z;
-  w.bar = (unsigned*)take(64);
-  w.DY = take(S * K1P * 32);
-  w.DGI1 = take(S * 3 * g.H * 32); w.DGH1 = take(S * 3 * g.H * 32);
-  w.DGI0 = take(S * 3 * g.H * 32); w.DGH0 = take(S * 3 * g.H * 32);
-  w.DPA = take(S * g.H * 32);
-  w.DH0 = take((size_t)g.nbt * g.H * 32); w.DH1 = take((size_t)g.nbt * g.H * 32);
-  w.COND = take(S * C * 32); w.DCOND = take(S * C * 32);
-  w.cse_dout = take((size_t)g.B * 2 * g.H); w.cse_d2 = take((size_t)g.B * g.H); w.cse_d1 = take((size_t)g.B * g.H);
-  w.cse_din = take((size_t)g.B * (P_IN + g.Z));
-  w.DCH = take((size_t)T * 32 * 8);
-  w.bytes = off;
+  w.bar = (unsigned*)a.take(64);
+  w.DY = a.take(S * K1P * 32);
+  w.DGI1 = a.take(S * 3 * g.H * 32); w.DGH1 = a.take(S * 3 * g.H * 32);
+  w.DGI0 = a.take(S * 3 * g.H * 32); w.DGH0 = a.take(S * 3 * g.H * 32);
+  w.DPA = a.take(S * g.H * 32);
+  w.DH0 = a.take((size_t)g.nbt * g.H * 32); w.DH1 = a.take((size_t)g.nbt * g.H * 32);
+  w.COND = a.take(S * C * 32); w.DCOND = a.take(S * C * 32);
+  w.cse_dout = a.take((size_t)g.B * 2 * g.H); w.cse_d2 = a.take((size_t)g.B * g.H); w.cse_d1 = a.take((size_t)g.B * g.H);
+  w.cse_din = a.take((size_t)g.B * (P_IN + g.Z));
+  w.DCH = a.take((size_t)T * 32 * 8);
+  w.bytes = a.off;
   return w;
 }
 
@@ -89,16 +84,15 @@ struct WgradHist { const float* src; long long stride; int rows; __nv_bfloat16 *
 struct WgradHists {
   WgradHist h[NHIST];
   int slots, nbt;     // slots per history (T * nbt), batch tiles
-  size_t ld, bytes;   // columns of every copy (slots * 32), bytes of all copies
-  char* end;          // first scratch byte behind them
+  size_t ld, bytes;   // columns of every copy (slots * 32), bytes of all copies (from the scratch base)
 };
 // The table and the carve-up, host arithmetic only: calls with the same geometry and scratch buffer return the same addresses.
 WgradHists wgrad_hists(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w,
                        const BwdWs& bw, bool want_lo);
 int split_hist(const WgradHists& hs, int i, cudaStream_t stream);
-// the six GEMMs; split-K partials go to the scratch bytes from `tail` on
+// the six GEMMs; split-K partials go to the rest of the scratch buffer behind `tail` (an arena over it)
 int wgrad_gemms(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const WgradHists& hs, bool want_lo,
-                char* tail, cudaStream_t stream);
+                Arena tail, cudaStream_t stream);
 int cond_kmajor(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdWs& bw, cudaStream_t stream);
 // CellStateEncoder backward (modules.py:238-243); its small GEMMs stage operands at the base of the scratch buffer
 int cse_backward(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecWs& w, const BwdWs& bw, cudaStream_t stream);

@@ -116,12 +116,11 @@ __global__ void pack_decoder_bwd_tc_kernel(DecGeom g, BtGeom tg, const float* __
 struct BtWs { uint8_t *g1img, *g0img, *dpaimg; const float* pre; float* dch; long long* dbg; size_t bytes; };
 long long* tc_debug_buffer();
 inline BtWs make_btws(void* base, const DecGeom& g) {
-  BtWs w; size_t off = 0;
-  auto take = [&](size_t n) { uint8_t* p = base ? (uint8_t*)base + off : nullptr; off += ((n + 1023) / 1024) * 1024; return p; };
+  BtWs w; Arena a{(char*)base, 0, 1024};
   const size_t kbH = ceil_div(g.H, 64);
-  w.g1img = take(kbH * 16384); w.g0img = take(kbH * 16384); w.dpaimg = take(kbH * 4096);
+  w.g1img = (uint8_t*)a.bytes(kbH * 16384); w.g0img = (uint8_t*)a.bytes(kbH * 16384); w.dpaimg = (uint8_t*)a.bytes(kbH * 4096);
   w.pre = nullptr; w.dch = nullptr; w.dbg = nullptr;
-  w.bytes = off; return w;
+  w.bytes = a.off; return w;
 }
 
 // trace of CTAs 0 and 1 (both ranks of pair 0): dbg[c][reverse step < 64][event < 32], clock64 of the CTA's SM
@@ -558,30 +557,8 @@ static int launch_bt(const zeggs_decoder_fwd_args& a, const DecGeom& g, const Bw
                      const BwdWs& bw, const BtWs& iw, const BwdArgsDev& d, const uint8_t* packed, cudaStream_t stream) {
   const size_t smem = 1024 + (size_t)BT_RING * tg.slot_bytes + 512 +
                       (size_t)((tg.N2 + tg.N3[1] + tg.N4) * BT_ACC_LD + 6 * U + 16) * sizeof(float);
-  // clusters of 2 CTAs (the pairs sharing an image), launched cooperatively: the kernel spins on a grid barrier, so every
-  // CTA must be resident at once
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeCooperative;
-  attr[1].val.cooperative = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(g.G); cfg.blockDim = dim3(224); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cfg.attrs = attr; cfg.numAttrs = 2;
-  static size_t checked_smem = 0;     // attribute + co-residency query once per shared-memory size (one device per process)
-  static int max_clusters = 0;
-  if (checked_smem != smem) {
-    ZCHECK_CUDA(cudaFuncSetAttribute(decoder_bwd_tc_kernel<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchConfig_t occ = cfg;
-    occ.numAttrs = 1;                 // the cluster shape only
-    ZCHECK_CUDA(cudaOccupancyMaxActiveClusters(&max_clusters, decoder_bwd_tc_kernel<U>, &occ));
-    checked_smem = smem;
-  }
-  ZCHECK_ARG(2 * max_clusters >= g.G, "decoder bwd tc: cooperative grid of %d CTAs in clusters of 2 does not fit (%d clusters resident)",
-             g.G, max_clusters);
-  ZCHECK_CUDA(cudaLaunchKernelEx(&cfg, decoder_bwd_tc_kernel<U>, a, g, bg, tg, w, bw, iw, d, packed));
-  count_launch();
-  return ZEGGS_OK;
+  // clusters of 2 CTAs: the pairs sharing an image
+  return launch_persistent(decoder_bwd_tc_kernel<U>, g.G, 224, smem, 2, stream, a, g, bg, tg, w, bw, iw, d, packed);
 }
 
 // Tensor-core engine backward.  Phase 0 runs all of it.  Phase 1 runs the BPTT recurrence, the CellStateEncoder backward and the
@@ -602,12 +579,11 @@ int decoder_window_bwd_tc(const zeggs_decoder_fwd_args& a, const zeggs_decoder_b
   // operands and result at the scratch base for the duration of the recurrence
   const int ldy = round_up(P_OUT, 8);
   const size_t rows = (size_t)a.B * T;
-  char* p = scratch_base();
-  auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) / 256 * 256; return r; };
-  __nv_bfloat16* dys = (__nv_bfloat16*)take(rows * ldy * 2);
-  __nv_bfloat16* w2t = (__nv_bfloat16*)take((size_t)H * ldy * 2);
-  float* pre = (float*)take(rows * H * sizeof(float));
-  ZCHECK_ARG((size_t)(p - scratch_base()) <= scratch_bytes(), "decoder bwd tc: scratch buffer too small (%zu bytes needed)", (size_t)(p - scratch_base()));
+  Arena st{scratch_base()};
+  __nv_bfloat16* dys = (__nv_bfloat16*)st.bytes(rows * ldy * 2);
+  __nv_bfloat16* w2t = (__nv_bfloat16*)st.bytes((size_t)H * ldy * 2);
+  float* pre = (float*)st.bytes(rows * H * sizeof(float));
+  ZCHECK_ARG(st.off <= scratch_bytes(), "decoder bwd tc: scratch buffer too small (%zu bytes needed)", st.off);
   // the weight gradients: single-pass bf16 history copies (the recurrence already runs on bf16 operands, so one pass matches its
   // accuracy), and behind them the dpa / dgi0 copies transposed to [(t,b)][row] (A operands of the d cond and x_pose gradient GEMMs),
   // the transposed cond / x_pose columns of W0 / W_ih0 and the DXP result
@@ -616,15 +592,14 @@ int decoder_window_bwd_tc(const zeggs_decoder_fwd_args& a, const zeggs_decoder_b
   const size_t extra = ld * H * 2 + ld * 3 * H * 2 + (size_t)C * 4 * H * 2 + (size_t)P_OUT * 4 * H * 2 + ld * P_OUT * 4 + 4096;
   ZCHECK_ARG(hs.bytes + extra <= scratch_bytes(), "decoder bwd tc: scratch buffer too small for the batched gradient GEMMs (%zu bytes needed)",
              hs.bytes + extra);
-  char* q = hs.end;
-  auto takeq = [&](size_t bytes) { char* r = (char*)(((uintptr_t)q + 255) & ~(uintptr_t)255); q = r + bytes; return r; };
-  __nv_bfloat16* paT = (__nv_bfloat16*)takeq(ld * H * 2);
-  __nv_bfloat16* giT = (__nv_bfloat16*)takeq(ld * 3 * H * 2);
-  __nv_bfloat16* w0T = (__nv_bfloat16*)takeq((size_t)C * H * 2);
-  __nv_bfloat16* wiT = (__nv_bfloat16*)takeq((size_t)C * 3 * H * 2);
-  __nv_bfloat16* w0xT = (__nv_bfloat16*)takeq((size_t)P_OUT * H * 2);
-  __nv_bfloat16* wixT = (__nv_bfloat16*)takeq((size_t)P_OUT * 3 * H * 2);
-  float* dxp = (float*)takeq(ld * P_OUT * 4);
+  Arena q{scratch_base(), hs.bytes, 1};   // each piece 256 B aligned, the split-K partials of wgrad_gemms behind the last
+  __nv_bfloat16* paT = (__nv_bfloat16*)q.align(256).bytes(ld * H * 2);
+  __nv_bfloat16* giT = (__nv_bfloat16*)q.align(256).bytes(ld * 3 * H * 2);
+  __nv_bfloat16* w0T = (__nv_bfloat16*)q.align(256).bytes((size_t)C * H * 2);
+  __nv_bfloat16* wiT = (__nv_bfloat16*)q.align(256).bytes((size_t)C * 3 * H * 2);
+  __nv_bfloat16* w0xT = (__nv_bfloat16*)q.align(256).bytes((size_t)P_OUT * H * 2);
+  __nv_bfloat16* wixT = (__nv_bfloat16*)q.align(256).bytes((size_t)P_OUT * 3 * H * 2);
+  float* dxp = (float*)q.align(256).bytes(ld * P_OUT * 4);
   const int cur = 32;                    // row of (t = 1, b = 0) in the transposed copies, column of slot t = 1 in the others
   const int Kc = (T - 1) * 32;
   int rc;

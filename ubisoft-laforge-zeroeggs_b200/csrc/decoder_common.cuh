@@ -1,65 +1,11 @@
 // Geometry, workspace layout and the weight-stationary "skinny GEMM" building block shared by the
 // decoder forward and backward persistent kernels.
 #pragma once
-#include "common.cuh"
-#include "../../include/zeggs_b200.h"
+#include "library.cuh"
 
 namespace zeggs {
 
 constexpr int K1P = 1136;  // P_IN (1134) rounded up to the 16-row k-chunk
-
-void count_launch();
-int timer_id(const char* name);
-void* timer_begin(int id, cudaStream_t s);
-void timer_end(void* h, cudaStream_t s);
-struct ScopedTimer {
-  void* h; cudaStream_t s;
-  ScopedTimer(const char* name, cudaStream_t st) : h(timer_begin(timer_id(name), st)), s(st) {}
-  ~ScopedTimer() { timer_end(h, s); }
-};
-int sgemm_launch(int trans_a, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
-                 const float* bias, float* C, int ldc, int act, int accumulate, cudaStream_t stream);
-int sgemm_batched_launch(int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
-                         const float* bias, float* C, int ldc, int act, int accumulate, int batch,
-                         long long sA, long long sB, long long sC, cudaStream_t stream);
-int gemm_f32_auto(int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb, const float* bias,
-                  float* C, int ldc, int act, int accumulate, cudaStream_t stream);
-const zeggs_ctx* swap_ctx(const zeggs_ctx* c);
-// RAII: the caller's context is the active one for the duration of one extern "C" entry point on this host thread
-struct CtxScope {
-  const zeggs_ctx* old; bool active;
-  explicit CtxScope(const zeggs_ctx* c) : old(nullptr), active(c != nullptr) { if (active) old = swap_ctx(c); }
-  ~CtxScope() { if (active) swap_ctx(old); }
-};
-int gemm_mode();
-char* scratch_base();
-size_t scratch_bytes();
-int split_hist_launch(const float* x, long long slot_stride, int S, int R, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t stream,
-                      float* rowsum = nullptr, int s_begin = 0);
-int transpose_bf16_launch(const __nv_bfloat16* in, int R, int Ncols, size_t ld_in, __nv_bfloat16* out, size_t ld_out, cudaStream_t stream);
-int split_t_launch(const float* x, int rows, int cols, int ld_in, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld_out, cudaStream_t stream);
-// convolution-as-GEMM on the tensor cores with the operand produced straight from x (tc_gemm.cu); ZEGGS_CONV_NOT_TAKEN = use the im2col path
-constexpr int ZEGGS_CONV_NOT_TAKEN = -1000;
-int conv_gemm_fwd(const float* x, int B, int T, int C, int k, int pad, int replicate, const float* W, const float* bias, float* y, int N,
-                  int act, cudaStream_t stream);
-int conv_gemm_wgrad(const float* dpre, int N, const float* x, int B, int T, int C, int k, int pad, int replicate, float* dW, cudaStream_t stream);
-int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, int lda,
-                   const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, const float* bias,
-                   float* C, int ldc, int act, int accumulate, cudaStream_t stream, float* splitk_ws = nullptr,
-                   size_t splitk_ws_bytes = 0);
-int sgemm_batched2_launch(int mode, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
-                          const float* bias, float* C, int ldc, int act, int accumulate, int batch,
-                          long long sA, long long sB, long long sC, int inner, long long iA, long long iB, long long iC,
-                          float alpha, cudaStream_t stream);
-// StyleEncoderGRU recurrences (style_gru.cu)
-int style_gru_units(int H);
-int style_gru_max_batch(int H);
-int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
-                         unsigned* bar, cudaStream_t s);
-int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs, const float* Gs, const float* dhf, int ld_dhf,
-                         float* dGih, float* dGhh, unsigned* bar, cudaStream_t s);
-int style_gru_rev_cell_fwd(int B, int H, const float* GIr, const float* bhh, float* hcat, cudaStream_t s);
-int style_gru_rev_cell_bwd(int B, int H, const float* GIr, const float* bhh, const float* dhcat, float* dGIr, float* dGHr, cudaStream_t s);
 
 // units per CTA: the grid G = H/U must fit one CTA per SM (132 on the H100 SXM).  At U = 16 the fp32 recurrences run each stage as
 // two passes of 8 units (pass_units), so the register tiles and shared-memory stages stay those of U = 8.
@@ -76,6 +22,8 @@ __host__ __device__ constexpr int pass_units(int U) { return U < 8 ? U : 8; }
 // hidden sizes the tensor-core recurrence (engine 1: forward and BPTT kernels) covers; every tc size / pack / run entry point
 // applies this one rule (the BPTT kernel pairs 64-wide k-blocks, and below 384 nothing has been validated)
 inline bool tc_hidden_ok(int H) { return H % 128 == 0 && H >= 384 && H <= 1024; }
+// hidden sizes the fp32 recurrences (engine 0, normal and FiLM) cover: every fp32 size / pack / run entry point applies this rule
+inline bool fp32_hidden_ok(int H) { return H % 16 == 0 && pick_U(H) > 0; }
 
 struct DecGeom {
   int B, H, S, Z, A;   // A = 1134 + S + Z
@@ -121,32 +69,27 @@ struct DecWs {
 
 inline DecWs make_ws(void* base, const DecGeom& g, int T, int save) {
   DecWs w;
-  size_t off = 0;
-  auto take = [&](size_t nfloats) {
-    float* p = base ? (float*)((char*)base + off) : nullptr;
-    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
-    return p;
-  };
+  Arena a{(char*)base};
   w.save = save ? 1 : 0;
   w.TS = save ? T : 2;
-  w.bar = (unsigned*)take(64);
-  w.cse_in = take((size_t)g.B * (P_IN + g.Z));
-  w.cse_h1 = take((size_t)g.B * g.H);
-  w.cse_h2 = take((size_t)g.B * g.H);
-  w.cse_out = take((size_t)g.B * 2 * g.H);
-  w.S01 = take((size_t)T * g.nbt * 4 * g.H * 32);
-  w.XP = take((size_t)(w.TS + 1) * g.nbt * K1P * 32);   // +1: step T-1 never writes slot T, keep the index math simple
-  w.A = take((size_t)w.TS * g.nbt * g.H * 32);
-  w.H0 = take((size_t)w.TS * g.nbt * g.H * 32);
-  w.H1 = take((size_t)w.TS * g.nbt * g.H * 32);
-  w.G0 = take(save ? (size_t)T * g.nbt * 4 * g.H * 32 : 64);
-  w.G1 = take(save ? (size_t)T * g.nbt * 4 * g.H * 32 : 64);
-  w.CONDR = take((size_t)T * g.nbt * 32 * (g.S + g.Z));
-  w.H1B = (void*)take((size_t)T * 32 * g.H / 2);
-  w.YC = take((size_t)T * 32 * P_OUT);
-  w.Y6 = take((size_t)T * 32 * 8);
-  w.GZ = take((size_t)T * 32 * 4);
-  w.bytes = off;
+  w.bar = (unsigned*)a.take(64);
+  w.cse_in = a.take((size_t)g.B * (P_IN + g.Z));
+  w.cse_h1 = a.take((size_t)g.B * g.H);
+  w.cse_h2 = a.take((size_t)g.B * g.H);
+  w.cse_out = a.take((size_t)g.B * 2 * g.H);
+  w.S01 = a.take((size_t)T * g.nbt * 4 * g.H * 32);
+  w.XP = a.take((size_t)(w.TS + 1) * g.nbt * K1P * 32);   // +1: step T-1 never writes slot T, keep the index math simple
+  w.A = a.take((size_t)w.TS * g.nbt * g.H * 32);
+  w.H0 = a.take((size_t)w.TS * g.nbt * g.H * 32);
+  w.H1 = a.take((size_t)w.TS * g.nbt * g.H * 32);
+  w.G0 = a.take(save ? (size_t)T * g.nbt * 4 * g.H * 32 : 64);
+  w.G1 = a.take(save ? (size_t)T * g.nbt * 4 * g.H * 32 : 64);
+  w.CONDR = a.take((size_t)T * g.nbt * 32 * (g.S + g.Z));
+  w.H1B = (void*)a.take((size_t)T * 32 * g.H / 2);
+  w.YC = a.take((size_t)T * 32 * P_OUT);
+  w.Y6 = a.take((size_t)T * 32 * 8);
+  w.GZ = a.take((size_t)T * 32 * 4);
+  w.bytes = a.off;
   return w;
 }
 
@@ -167,17 +110,12 @@ __host__ __device__ constexpr int film_rows(int U) { return U < 8 ? 8 : U; }
 // FiLM forward workspace: the normal decoder's carve-up followed by GB, E0, E2, C2; bytes = the whole workspace
 inline FilmDev make_film_ws(void* base, const DecWs& w, const DecGeom& g, int T, size_t* bytes) {
   FilmDev f = {};
-  size_t off = w.bytes;
-  auto take = [&](size_t nfloats) {
-    float* p = base ? (float*)((char*)base + off) : nullptr;
-    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
-    return p;
-  };
-  f.GB = take((size_t)g.B * T * 4 * g.H);
-  f.E0 = take(w.save ? (size_t)T * g.nbt * g.H * 32 : 64);
-  f.E2 = take(w.save ? (size_t)T * g.nbt * g.H * 32 : 64);
-  f.C2 = take((size_t)w.TS * g.nbt * g.H * 32);
-  *bytes = off;
+  Arena a{(char*)base, w.bytes};
+  f.GB = a.take((size_t)g.B * T * 4 * g.H);
+  f.E0 = a.take(w.save ? (size_t)T * g.nbt * g.H * 32 : 64);
+  f.E2 = a.take(w.save ? (size_t)T * g.nbt * g.H * 32 : 64);
+  f.C2 = a.take((size_t)w.TS * g.nbt * g.H * 32);
+  *bytes = a.off;
   return f;
 }
 

@@ -344,25 +344,22 @@ static size_t fwd_smem_bytes(int nbt) {
 static int check_fwd_args(const zeggs_decoder_fwd_args* a) {
   ZCHECK_ARG(a != nullptr, "decoder: null args");
   ZCHECK_ARG(a->B >= 1 && a->T >= 1, "decoder: bad B=%d T=%d", a->B, a->T);
-  ZCHECK_ARG(a->H % 16 == 0 && pick_U(a->H) > 0, "decoder: hidden size %d unsupported (need H%%16==0, H<=2112)", a->H);
+  ZCHECK_ARG(fp32_hidden_ok(a->H), "decoder: hidden size %d unsupported (need H%%16==0, H<=2112)", a->H);
   ZCHECK_ARG(a->S >= 1 && a->Z >= 1 && a->S + a->Z <= 256, "decoder: bad S=%d Z=%d", a->S, a->Z);
   if (a->engine != 1) {
     const int U = pick_U(a->H);
     size_t (*smem_of)(int) = U == 4 ? fwd_smem_bytes<4> : U == 8 ? fwd_smem_bytes<8> : fwd_smem_bytes<16>;
     const int nbt = ceil_div(a->B, 32);
-    int dev = 0, cap = 0;
-    ZCHECK_CUDA(cudaGetDevice(&dev));
-    ZCHECK_CUDA(cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    int max_nbt = nbt;
-    while (max_nbt > 0 && smem_of(max_nbt) > (size_t)cap) --max_nbt;
-    ZCHECK_ARG(smem_of(nbt) <= (size_t)cap, "decoder: batch %d needs %zu bytes of shared memory per CTA at hidden size %d (%d available): at "
-               "most %d samples per call", a->B, smem_of(nbt), a->H, cap, 32 * max_nbt);
+    DeviceLimits lim;
+    RC(device_limits(&lim));
+    ZCHECK_ARG(smem_of(nbt) <= lim.smem_optin, "decoder: batch %d needs %zu bytes of shared memory per CTA at hidden size %d (%zu available): "
+               "at most %d samples per call", a->B, smem_of(nbt), a->H, lim.smem_optin, 32 * max_batch_tiles(smem_of, lim.smem_optin));
   }
   return ZEGGS_OK;
 }
 
 extern "C" size_t zeggs_decoder_packed_bytes(int H, int S, int Z) {
-  if (H % 16 != 0 || pick_U(H) <= 0) return 0;
+  if (!fp32_hidden_ok(H)) return 0;
   DecGeom g = make_geom(1, H, S, Z);
   return g.packed_floats() * sizeof(float);
 }
@@ -379,31 +376,22 @@ extern "C" int zeggs_decoder_pack_weights(const zeggs_decoder_fwd_args* a, float
 }
 
 extern "C" size_t zeggs_decoder_workspace_bytes(int B, int T, int H, int S, int Z, int save) {
-  if (H % 16 != 0 || pick_U(H) <= 0 || B < 1 || T < 1) return 0;
+  if (!fp32_hidden_ok(H) || B < 1 || T < 1) return 0;
   DecGeom g = make_geom(B, H, S, Z);
   return make_ws(nullptr, g, T, save).bytes;
 }
 
 template <int U, bool FILM>
 static int launch_fwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, const FilmDev& f, cudaStream_t stream) {
-  const size_t smem = fwd_smem_bytes<U>(g.nbt);            // within the device's limit: check_fwd_args
-  ZCHECK_CUDA(cudaFuncSetAttribute(decoder_fwd_kernel<U, FILM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int dev = 0, nsm = 0, occ = 0;
-  ZCHECK_CUDA(cudaGetDevice(&dev));
-  ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_fwd_kernel<U, FILM>, 256, smem));
-  ZCHECK_ARG(occ * nsm >= g.G, "decoder: cooperative grid of %d CTAs does not fit (%d SMs x %d)", g.G, nsm, occ);
-  void* args[] = {(void*)&a, (void*)&g, (void*)&w, (void*)&f};
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_fwd_kernel<U, FILM>, dim3(g.G), dim3(256), args, smem, stream));
-  count_launch();
-  return ZEGGS_OK;
+  // the shared memory is within the device's limit: check_fwd_args
+  return launch_persistent(decoder_fwd_kernel<U, FILM>, g.G, 256, fwd_smem_bytes<U>(g.nbt), 1, stream, a, g, w, f);
 }
 
 // fp32 engine: the hoisted speech / style terms, then the SIMT recurrence
 static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
   const int C = a.S + a.Z;
   const size_t sm = (size_t)(C * 33 + 64 * (C + 1)) * sizeof(float);
-  ZCHECK_CUDA(cudaFuncSetAttribute(cond_precompute_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  RC(set_max_dynamic_smem(cond_precompute_kernel, sm));
   cond_precompute_kernel<<<dim3(a.T, g.nbt, ceil_div(4 * a.H, 64)), 256, sm, stream>>>(a, g, w.S01);
   count_launch();
   ZCHECK_LAUNCH();
@@ -472,7 +460,7 @@ static int check_film_args(const zeggs_decoder_film_fwd_args* f) {
 static size_t film_packed_floats(const DecGeom& g) { return g.packed_floats() + (size_t)g.G * g.H * film_rows(g.U); }
 
 extern "C" size_t zeggs_decoder_packed_film_bytes(int H, int S, int Z) {
-  if (H % 16 != 0 || pick_U(H) <= 0) return 0;
+  if (!fp32_hidden_ok(H)) return 0;
   return film_packed_floats(make_film_geom(1, H, S, Z)) * sizeof(float);
 }
 
@@ -491,7 +479,7 @@ extern "C" int zeggs_decoder_pack_weights_film(const zeggs_decoder_film_fwd_args
 }
 
 extern "C" size_t zeggs_decoder_film_workspace_bytes(int B, int T, int H, int S, int Z, int save) {
-  if (H % 16 != 0 || pick_U(H) <= 0 || B < 1 || T < 1) return 0;
+  if (!fp32_hidden_ok(H) || B < 1 || T < 1) return 0;
   DecGeom g = make_film_geom(B, H, S, Z);
   size_t bytes = 0;
   make_film_ws(nullptr, make_ws(nullptr, g, T, save), g, T, &bytes);
@@ -520,7 +508,7 @@ extern "C" int zeggs_decoder_film_window_fwd(const zeggs_decoder_film_fwd_args* 
   zeggs_decoder_fwd_args as = a;
   as.Z = 0;
   const size_t sm = (size_t)(a.S * 33 + 64 * (a.S + 1)) * sizeof(float);
-  ZCHECK_CUDA(cudaFuncSetAttribute(cond_precompute_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  RC(set_max_dynamic_smem(cond_precompute_kernel, sm));
   cond_precompute_kernel<<<dim3(a.T, g.nbt, ceil_div(4 * a.H, 64)), 256, sm, stream>>>(as, g, w.S01);
   count_launch();
   ZCHECK_LAUNCH();

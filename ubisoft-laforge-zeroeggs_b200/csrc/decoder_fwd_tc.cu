@@ -185,13 +185,12 @@ struct TcWs {
   size_t bytes;
 };
 inline TcWs make_tcws(void* base, const DecGeom& g) {
-  TcWs w; size_t off = 0;
-  auto take = [&](size_t n) { uint8_t* p = base ? (uint8_t*)base + off : nullptr; off += ((n + 1023) / 1024) * 1024; return p; };
+  TcWs w; Arena a{(char*)base, 0, 1024};
   const size_t hb = (size_t)ceil_div(g.H, 64) * 4096;
-  w.ab = take(hb);
-  w.h0b[0] = take(hb); w.h0b[1] = take(hb); w.h1b[0] = take(hb); w.h1b[1] = take(hb);
+  w.ab = (uint8_t*)a.bytes(hb);
+  w.h0b[0] = (uint8_t*)a.bytes(hb); w.h0b[1] = (uint8_t*)a.bytes(hb); w.h1b[0] = (uint8_t*)a.bytes(hb); w.h1b[1] = (uint8_t*)a.bytes(hb);
   w.dbg = nullptr;
-  w.bytes = off; return w;
+  w.bytes = a.off; return w;
 }
 
 // per-CTA phase timestamps (development trace): dbg[(cta * 64 + t) * 32 + event], SM-local clock64
@@ -691,21 +690,7 @@ static int launch_tc(const zeggs_decoder_fwd_args& a, const DecGeom& g, const Tc
                      const uint8_t* packed, cudaStream_t stream) {
   const size_t smem = 1024 + (size_t)2 * tg.kbH * 4096 + (size_t)TC_RING * tg.slot_bytes + 4096 + 512 +
                       (size_t)(28 * U + 26 + (2 * tg.NP + tg.N1) * TC_ACC_LD) * sizeof(float);
-  constexpr int NT = 256;
-  static size_t checked_smem = 0;     // attribute + co-residency check once per shared-memory size (one device per process)
-  if (checked_smem != smem) {
-    ZCHECK_CUDA(cudaFuncSetAttribute(decoder_fwd_tc_kernel<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, nsm = 0, occ = 0;
-    ZCHECK_CUDA(cudaGetDevice(&dev));
-    ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-    ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decoder_fwd_tc_kernel<U>, NT, smem));
-    ZCHECK_ARG(occ * nsm >= g.G, "decoder tc: cooperative grid of %d CTAs does not fit", g.G);
-    checked_smem = smem;
-  }
-  void* args[] = {(void*)&a, (void*)&g, (void*)&tg, (void*)&w, (void*)&tw, (void*)&packed};
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)decoder_fwd_tc_kernel<U>, dim3(g.G), dim3(NT), args, smem, stream));
-  count_launch();
-  return ZEGGS_OK;
+  return launch_persistent(decoder_fwd_tc_kernel<U>, g.G, 256, smem, 1, stream, a, g, tg, w, tw, packed);
 }
 
 const float* decoder_tc_mfold(const zeggs_decoder_fwd_args& a) {

@@ -31,10 +31,9 @@ __global__ void step_gru_kernel(int B, int H, const float* __restrict__ gi, cons
 
 struct StepWs { float *v, *gi, *gh; size_t bytes; };
 static StepWs step_ws(void* base, int B, int H, int S, int Z) {
-  StepWs w; size_t off = 0;
-  auto take = [&](size_t n) { float* p = base ? (float*)((char*)base + off) : nullptr; off += ((n * 4 + 255) / 256) * 256; return p; };
-  w.v = take((size_t)B * (H + P_IN + S + Z)); w.gi = take((size_t)B * 3 * H); w.gh = take((size_t)B * 3 * H);
-  w.bytes = off; return w;
+  StepWs w; Arena a{(char*)base};
+  w.v = a.take((size_t)B * (H + P_IN + S + Z)); w.gi = a.take((size_t)B * 3 * H); w.gh = a.take((size_t)B * 3 * H);
+  w.bytes = a.off; return w;
 }
 extern "C" size_t zeggs_decoder_step_workspace_bytes(int B, int H, int S, int Z) {
   return (B < 1 || H < 1) ? 0 : step_ws(nullptr, B, H, S, Z).bytes;

@@ -4,7 +4,7 @@
 // pooling and the VAE sample are small row-wise kernels.  One C-ABI call per module direction; all
 // intermediates live in the caller's workspace (they are the "saved tensors" of the backward).
 // Dropout masks are explicit multiplier tensors (0 or 1/(1-p)) supplied by the caller (NULL = eval mode).
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 
@@ -238,17 +238,7 @@ __global__ void vae_sample_bwd_kernel(const float* __restrict__ dz, const float*
   dpooled[(size_t)b * 2 * Z + Z + j] = gl;
 }
 // ------------------------------------------------------------------ launch helpers
-struct Arena {
-  char* base; size_t off;
-  float* take(size_t nfloats) {
-    float* p = base ? (float*)(base + off) : nullptr;
-    off += ((nfloats * sizeof(float) + 255) / 256) * (size_t)256;
-    return p;
-  }
-};
 #define GRID1(n) (unsigned)((((size_t)(n) + 255) / 256) > 4736 ? 4736 : (((size_t)(n) + 255) / 256))
-#define LAUNCH_OK() do { count_launch(); ZCHECK_LAUNCH(); } while (0)
-#define RC(x) do { int _rc = (x); if (_rc) return _rc; } while (0)
 
 static int im2col(const float* x, int B, int T, int C, int k, int pad, int rep, float* col, cudaStream_t s) {
   im2col_kernel<<<GRID1((size_t)B * T * C * k), 256, 0, s>>>(x, B, T, C, k, pad, rep, col); LAUNCH_OK(); return 0; }
@@ -260,26 +250,29 @@ static int ew_add(float* dst, const float* a, const float* b, size_t n, size_t p
   ew_add_kernel<<<GRID1(n), 256, 0, s>>>(dst, a, b, n, period); LAUNCH_OK(); return 0; }
 static int ln_fwd(const float* a, const float* res, const float* g, const float* b, int rows, int D, float* y, float* xh, float* rs, cudaStream_t s) {
   layernorm_fwd_kernel<<<ceil_div(rows, 8), 256, 0, s>>>(a, res, g, b, rows, D, y, xh, rs); LAUNCH_OK(); return 0; }
-static thread_local float* g_redbuf = nullptr;   // [COLRED_RB][2][D <= 4096] scratch inside the calling module's workspace (per host thread: re-entrant)
-static int colred(const float* a, const float* b, int rows, int D, float* out0, float* out1, cudaStream_t s) {
-  ZCHECK_ARG(g_redbuf != nullptr && D <= COLRED_MAXD, "column reduction: scratch missing or D=%d too wide", D);
+// red: the column reductions' scratch inside the calling module's workspace, [COLRED_RB][2][D <= 4096] partials + arrival counters
+static int colred(const float* a, const float* b, int rows, int D, float* out0, float* out1, float* red, cudaStream_t s) {
+  ZCHECK_ARG(red != nullptr && D <= COLRED_MAXD, "column reduction: scratch missing or D=%d too wide", D);
   const int RB = rows < 8 * COLRED_RB ? ceil_div(rows, 8) : COLRED_RB;
-  int* counters = reinterpret_cast<int*>(g_redbuf + (size_t)COLRED_RB * 2 * COLRED_MAXD);
-  colred_kernel<<<dim3(ceil_div(D, 32), RB), dim3(32, 8), 0, s>>>(a, b, rows, D, g_redbuf, counters, out0, out1); LAUNCH_OK(); return 0; }
+  int* counters = reinterpret_cast<int*>(red + (size_t)COLRED_RB * 2 * COLRED_MAXD);
+  colred_kernel<<<dim3(ceil_div(D, 32), RB), dim3(32, 8), 0, s>>>(a, b, rows, D, red, counters, out0, out1); LAUNCH_OK(); return 0; }
 // the arrival counters behind the partials must be zero before the first reduction of a call (the workspace is caller memory)
-static int colred_reset(cudaStream_t s) {
-  ZCHECK_CUDA(cudaMemsetAsync(g_redbuf + (size_t)COLRED_RB * 2 * COLRED_MAXD, 0, (COLRED_MAXD / 32) * sizeof(int), s)); return 0; }
-static int ln_bwd(const float* dy, const float* xh, const float* rs, const float* g, int rows, int D, float* dx, float* dg, float* db, cudaStream_t s) {
+static int colred_reset(float* red, cudaStream_t s) {
+  ZCHECK_CUDA(cudaMemsetAsync(red + (size_t)COLRED_RB * 2 * COLRED_MAXD, 0, (COLRED_MAXD / 32) * sizeof(int), s)); return 0; }
+static int ln_bwd(const float* dy, const float* xh, const float* rs, const float* g, int rows, int D, float* dx, float* dg, float* db,
+                  float* red, cudaStream_t s) {
   layernorm_bwd_kernel<<<ceil_div(rows, 8), 256, 0, s>>>(dy, xh, rs, g, rows, D, dx); LAUNCH_OK();
-  return colred(dy, xh, rows, D, dg, db, s); }
-static int colsum(const float* x, int rows, int cols, float* out, cudaStream_t s) { return colred(x, nullptr, rows, cols, out, nullptr, s); }
+  return colred(dy, xh, rows, D, dg, db, red, s); }
+static int colsum(const float* x, int rows, int cols, float* out, float* red, cudaStream_t s) {
+  return colred(x, nullptr, rows, cols, out, nullptr, red, s); }
 // Linear / conv-as-GEMM forward: y[M,N] = act(x[M,K] W[N,K]^T + b)
 static int lin_fwd(const float* x, const float* W, const float* b, float* y, int M, int N, int K, int act, cudaStream_t s) {
   return gemm_f32_auto(0, M, N, K, x, K, W, K, b, y, N, act, 0, s); }
 // backward of y = x W^T + b given dpre[M,N]:  dW[N,K] = dpre^T x ; db ; dx[M,K] = dpre W (optional)
-static int lin_bwd(const float* dpre, const float* x, const float* W, float* dW, float* db, float* dx, int M, int N, int K, cudaStream_t s) {
+static int lin_bwd(const float* dpre, const float* x, const float* W, float* dW, float* db, float* dx, int M, int N, int K, float* red,
+                   cudaStream_t s) {
   RC(gemm_f32_auto(1, N, K, M, dpre, N, x, K, nullptr, dW, K, 0, 0, s));
-  if (db) RC(colsum(dpre, M, N, db, s));
+  if (db) RC(colsum(dpre, M, N, db, red, s));
   if (dx) RC(gemm_f32_auto(2, M, K, N, dpre, N, W, K, nullptr, dx, K, 0, 0, s));
   return 0;
 }
@@ -295,7 +288,7 @@ static int conv_fwd(const float* x, int B, int T, int C, int k, int pad, int rep
 }
 // backward given dpre[(b,t)][N]: dW, db, and (optional) dcol[(b,t)][C*k] = dpre W for col2im
 static int conv_bwd(const float* dpre, const float* x, int B, int T, int C, int k, int pad, int rep, const float* W, float* dW, float* db,
-                    float* dcol, int N, float* col, cudaStream_t s) {
+                    float* dcol, int N, float* col, float* red, cudaStream_t s) {
   const int M = B * T, K = C * k;
   int rc = conv_gemm_wgrad(dpre, N, x, B, T, C, k, pad, rep, dW, s);
   if (rc == ZEGGS_CONV_NOT_TAKEN) {
@@ -303,7 +296,7 @@ static int conv_bwd(const float* dpre, const float* x, int B, int T, int C, int 
     rc = gemm_f32_auto(1, N, K, M, dpre, N, col, K, nullptr, dW, K, 0, 0, s);
   }
   if (rc) return rc;
-  if (db) RC(colsum(dpre, M, N, db, s));
+  if (db) RC(colsum(dpre, M, N, db, red, s));
   if (dcol) RC(gemm_f32_auto(2, M, K, N, dpre, N, W, K, nullptr, dcol, K, 0, 0, s));
   return 0;
 }
@@ -344,16 +337,15 @@ extern "C" int zeggs_speech_enc_bwd(const zeggs_speech_enc_args* ap, const zeggs
   const zeggs_speech_enc_args& a = *ap; const zeggs_speech_enc_grads& g = *gp; cudaStream_t s = (cudaStream_t)stream_;
   const int B = a.B, T = a.T, Cin = a.C_in, H = a.H, O = a.O, k = 31, M = B * T;
   SpeechWs w = speech_ws(a.workspace, B, T, Cin, H, O, k);
-  g_redbuf = w.red;
-  RC(colred_reset(s));
+  RC(colred_reset(w.red, s));
   ScopedTimer tm("encoders_bwd", s);
   RC(ew_mul(w.t0, g.dy, nullptr, a.y, 1, (size_t)M * O, s));                        // dpre2 = dy * ELU'(y)
-  RC(lin_bwd(w.t0, w.h1d, a.W2, g.dW2, g.db2, w.t1, M, O, O, s));                   // t1 = d h1d
+  RC(lin_bwd(w.t0, w.h1d, a.W2, g.dW2, g.db2, w.t1, M, O, O, w.red, s));            // t1 = d h1d
   RC(ew_mul(w.t0, w.t1, a.mask1, w.h1, 1, (size_t)M * O, s));                       // dpre1
-  RC(conv_bwd(w.t0, w.h0d, B, T, H, k, k / 2, 1, a.W1, g.dW1, g.db1, w.dcol, O, w.col1, s));   // dW1, db1, dcol1
+  RC(conv_bwd(w.t0, w.h0d, B, T, H, k, k / 2, 1, a.W1, g.dW1, g.db1, w.dcol, O, w.col1, w.red, s)); // dW1, db1, dcol1
   RC(col2im(w.dcol, B, T, H, k, k / 2, 1, w.t1, s));                                // d h0d
   RC(ew_mul(w.t0, w.t1, a.mask0, w.h0, 1, (size_t)M * H, s));                       // dpre0
-  RC(lin_bwd(w.t0, a.x, a.W0, g.dW0, g.db0, nullptr, M, H, Cin, s));
+  RC(lin_bwd(w.t0, a.x, a.W0, g.dW0, g.db0, nullptr, M, H, Cin, w.red, s));
   return ZEGGS_OK;
 }
 
@@ -441,8 +433,7 @@ extern "C" int zeggs_style_enc_bwd(const zeggs_style_enc_args* ap, const zeggs_s
   const size_t nE = (size_t)M * E;
   const bool vae = a.mu != nullptr;
   ZCHECK_ARG(vae || (g.dz && !g.dmu && !g.dlogvar), "style_enc bwd: without the VAE (mu == NULL) dz [B,E] is required and dmu / dlogvar must be NULL");
-  g_redbuf = w.red;
-  RC(colred_reset(s));
+  RC(colred_reset(w.red, s));
   ScopedTimer tm("encoders_bwd", s);
   // VAE sample + mean pool
   if (vae) {
@@ -450,18 +441,18 @@ extern "C" int zeggs_style_enc_bwd(const zeggs_style_enc_args* ap, const zeggs_s
   }
   meanpool_bwd_kernel<<<GRID1(nE), 256, 0, s>>>(vae ? w.pooled : g.dz, B, T, E, w.g0); LAUNCH_OK();  // g0 = d x2
   // x2 = LN4(f2d + x1)
-  RC(ln_bwd(w.g0, w.xh4, w.rs4, a.ln4_g, M, E, w.g1, g.dln4_g, g.dln4_b, s));                        // g1 = d(f2d + x1)
+  RC(ln_bwd(w.g0, w.xh4, w.rs4, a.ln4_g, M, E, w.g1, g.dln4_g, g.dln4_b, w.red, s));                 // g1 = d(f2d + x1)
   RC(ew_mul(w.g0, w.g1, a.mask_ff, nullptr, 0, nE, s));                                              // g0 = d f2 (pre-act, linear)
-  RC(conv_bwd(w.g0, w.f1, B, T, E, 3, 1, 0, a.Wf2, g.dWf2, g.dbf2, w.gcol, E, w.colf2, s));
+  RC(conv_bwd(w.g0, w.f1, B, T, E, 3, 1, 0, a.Wf2, g.dWf2, g.dbf2, w.gcol, E, w.colf2, w.red, s));
   RC(col2im(w.gcol, B, T, E, 3, 1, 0, w.g0, s));                                                     // g0 = d f1
   RC(ew_mul(w.g0, w.g0, nullptr, w.f1, 2, nE, s));                                                   // ReLU'
-  RC(conv_bwd(w.g0, w.x1, B, T, E, 3, 1, 0, a.Wf1, g.dWf1, g.dbf1, w.gcol, E, w.colf, s));
+  RC(conv_bwd(w.g0, w.x1, B, T, E, 3, 1, 0, a.Wf1, g.dWf1, g.dbf1, w.gcol, E, w.colf, w.red, s));
   RC(col2im(w.gcol, B, T, E, 3, 1, 0, w.g0, s));                                                     // g0 = d x1 via FF
   RC(ew_add(w.g1, w.g1, w.g0, nE, 0, s));                                                            // g1 = total d x1
   // x1 = LN3(aod + x0)
-  RC(ln_bwd(w.g1, w.xh3, w.rs3, a.ln3_g, M, E, w.g2, g.dln3_g, g.dln3_b, s));                        // g2 = d(aod + x0)
+  RC(ln_bwd(w.g1, w.xh3, w.rs3, a.ln3_g, M, E, w.g2, g.dln3_g, g.dln3_b, w.red, s));                 // g2 = d(aod + x0)
   RC(ew_mul(w.g0, w.g2, a.mask_ao, nullptr, 0, nE, s));                                              // g0 = d ao
-  RC(lin_bwd(w.g0, w.o, a.Wout, g.dWout, g.dbout, w.g1, M, E, E, s));                                // g1 = d o
+  RC(lin_bwd(w.g0, w.o, a.Wout, g.dWout, g.dbout, w.g1, M, E, E, w.red, s));                         // g1 = d o
   // attention: o = Pd v ; Pd = softmax(S) * mask ; S = scale q k^T
   float* dPd = w.S;   // S is dead after the forward softmax: reuse for dPd / dS
   RC(sgemm_batched2_launch(0, T, T, d, w.g1, E, w.qkv + 2 * E, 3 * E, nullptr, dPd, T, 0, 0, B * nh,
@@ -474,18 +465,18 @@ extern "C" int zeggs_style_enc_bwd(const zeggs_style_enc_args* ap, const zeggs_s
                            nh * TT, (long long)T * 3 * E, (long long)T * 3 * E, nh, TT, d, d, sc, s));  // dq = scale dS k
   RC(sgemm_batched2_launch(1, T, d, T, dPd, T, w.qkv, 3 * E, nullptr, w.gqkv + E, 3 * E, 0, 0, B * nh,
                            nh * TT, (long long)T * 3 * E, (long long)T * 3 * E, nh, TT, d, d, sc, s));  // dk = scale dS^T q
-  RC(lin_bwd(w.gqkv, w.x0, a.Win, g.dWin, g.dbin, w.g0, M, 3 * E, E, s));                             // g0 = d x0 via qkv
+  RC(lin_bwd(w.gqkv, w.x0, a.Win, g.dWin, g.dbin, w.g0, M, 3 * E, E, w.red, s));                      // g0 = d x0 via qkv
   RC(ew_add(w.g2, w.g2, w.g0, nE, 0, s));                                                            // g2 = total d x0 = d l2d
   // conv stack
   RC(ew_mul(w.g0, w.g2, a.mask_c2, nullptr, 0, nE, s));                                              // d l2
-  RC(ln_bwd(w.g0, w.xh2, w.rs2, a.ln2_g, M, E, w.g1, g.dln2_g, g.dln2_b, s));                        // g1 = d c2
+  RC(ln_bwd(w.g0, w.xh2, w.rs2, a.ln2_g, M, E, w.g1, g.dln2_g, g.dln2_b, w.red, s));                 // g1 = d c2
   RC(ew_mul(w.g1, w.g1, nullptr, w.c2, 2, nE, s));
-  RC(conv_bwd(w.g1, w.l1d, B, T, Hs, 3, 1, 0, a.Wc2, g.dWc2, g.dbc2, w.gcol, E, w.col1, s));
+  RC(conv_bwd(w.g1, w.l1d, B, T, Hs, 3, 1, 0, a.Wc2, g.dWc2, g.dbc2, w.gcol, E, w.col1, w.red, s));
   RC(col2im(w.gcol, B, T, Hs, 3, 1, 0, w.g0, s));                                                    // g0 = d l1d
   RC(ew_mul(w.g0, w.g0, a.mask_c1, nullptr, 0, (size_t)M * Hs, s));
-  RC(ln_bwd(w.g0, w.xh1, w.rs1, a.ln1_g, M, Hs, w.g1, g.dln1_g, g.dln1_b, s));                       // g1 = d c1
+  RC(ln_bwd(w.g0, w.xh1, w.rs1, a.ln1_g, M, Hs, w.g1, g.dln1_g, g.dln1_b, w.red, s));                // g1 = d c1
   RC(ew_mul(w.g1, w.g1, nullptr, w.c1, 2, (size_t)M * Hs, s));
-  RC(conv_bwd(w.g1, a.x, B, T, Cin, 3, 1, 0, a.Wc1, g.dWc1, g.dbc1, nullptr, Hs, w.col0, s));
+  RC(conv_bwd(w.g1, a.x, B, T, Cin, 3, 1, 0, a.Wc1, g.dWc1, g.dbc1, nullptr, Hs, w.col0, w.red, s));
   return ZEGGS_OK;
 }
 
@@ -562,33 +553,32 @@ extern "C" int zeggs_style_enc_gru_bwd(const zeggs_style_enc_gru_args* ap, const
              "samples per call", B, H, style_gru_max_batch(H));
   StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);
   ZCHECK_ARG(a.workspace && a.workspace_bytes >= w.bytes, "style_enc_gru bwd: workspace too small");
-  g_redbuf = w.red;
-  RC(colred_reset(s));
+  RC(colred_reset(w.red, s));
   ScopedTimer tm("encoders_bwd", s);
   const float* dproj = g.dz;
   if (vae) {
     vae_sample_bwd_kernel<<<ceil_div(B * (E / 2), 256), 256, 0, s>>>(g.dz, g.dmu, g.dlogvar, a.eps, a.logvar, B, E / 2, 1.0f / a.temperature, w.dpooled); LAUNCH_OK();
     dproj = w.dpooled;
   }
-  RC(lin_bwd(dproj, w.hcat, a.Wp, g.dWp, g.dbp, w.dhcat, B, E, 2 * H, s));                          // dhcat = d output[:, -1]
+  RC(lin_bwd(dproj, w.hcat, a.Wp, g.dWp, g.dbp, w.dhcat, B, E, 2 * H, w.red, s));                   // dhcat = d output[:, -1]
   // reverse cell at T-1: W_ih_r / b_ih_r / b_hh_r gradients, W_hh_r's is zero (it multiplied h = 0)
   RC(style_gru_rev_cell_bwd(B, H, w.GIr, a.b_hh_r, w.dhcat, w.dGIr, w.dGHr, s));
   RC(gemm_f32_auto(1, 3 * H, H, B, w.dGIr, 3 * H, w.c2 + (size_t)(T - 1) * H, T * H, nullptr, g.dW_ih_r, H, 0, 0, s));
-  RC(colsum(w.dGIr, B, 3 * H, g.db_ih_r, s));
-  RC(colsum(w.dGHr, B, 3 * H, g.db_hh_r, s));
+  RC(colsum(w.dGIr, B, 3 * H, g.db_ih_r, w.red, s));
+  RC(colsum(w.dGHr, B, 3 * H, g.db_hh_r, w.red, s));
   ZCHECK_CUDA(cudaMemsetAsync(g.dW_hh_r, 0, (size_t)3 * H * H * sizeof(float), s));
   // forward direction: BPTT, then every weight / bias / input gradient as a GEMM or column sum over all (t, b)
   RC(style_gru_bwd_launch(B, T, H, a.W_hh, w.Hs, w.Gs, w.dhcat, 2 * H, w.dGih, w.dGhh, w.bar, s));
   RC(gemm_f32_auto(1, 3 * H, H, M, w.dGhh, 3 * H, w.Hs, H, nullptr, g.dW_hh, H, 0, 0, s));            // sum_t dG_hh(t)^T h(t-1)
-  RC(colsum(w.dGhh, M, 3 * H, g.db_hh, s));
-  RC(lin_bwd(w.dGih, w.c2, a.W_ih, g.dW_ih, g.db_ih, w.dc2, M, 3 * H, H, s));
+  RC(colsum(w.dGhh, M, 3 * H, g.db_hh, w.red, s));
+  RC(lin_bwd(w.dGih, w.c2, a.W_ih, g.dW_ih, g.db_ih, w.dc2, M, 3 * H, H, w.red, s));
   RC(gemm_f32_auto(2, B, H, 3 * H, w.dGIr, 3 * H, a.W_ih_r, H, nullptr, w.dc2 + (size_t)(T - 1) * H, T * H, 0, 1, s));   // + reverse cell
   // convs
   RC(ew_mul(w.dc2, w.dc2, nullptr, w.c2, 2, (size_t)M * H, s));
-  RC(conv_bwd(w.dc2, w.c1, B, T, H, 3, 1, 0, a.Wc2, g.dWc2, g.dbc2, w.gcol, H, w.col1, s));
+  RC(conv_bwd(w.dc2, w.c1, B, T, H, 3, 1, 0, a.Wc2, g.dWc2, g.dbc2, w.gcol, H, w.col1, w.red, s));
   RC(col2im(w.gcol, B, T, H, 3, 1, 0, w.dc1, s));
   RC(ew_mul(w.dc1, w.dc1, nullptr, w.c1, 2, (size_t)M * H, s));
-  RC(conv_bwd(w.dc1, a.x, B, T, Cin, 3, 1, 0, a.Wc1, g.dWc1, g.dbc1, nullptr, H, w.col0, s));
+  RC(conv_bwd(w.dc1, a.x, B, T, Cin, 3, 1, 0, a.Wc1, g.dWc1, g.dbc1, nullptr, H, w.col0, w.red, s));
   return ZEGGS_OK;
 }
 

@@ -4,7 +4,7 @@
 // (rows [ex_start, ex_start + ex_n) of the six pose arrays concatenated to 1134 channels with a zero gaze slot, then -- when the
 // example is shorter than L -- its own last L - ex_n rows again, dataset.py:198-203).  Pure row copies: bit-exact, HBM bound
 // (every output byte written once, every input byte read once; rows are contiguous so all accesses are coalesced).
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 

@@ -3,7 +3,7 @@
 //   trans_a = 1:  C[M,N] = A[K,M]^T * B[K,N] (+ C)           (weight gradients, contraction over rows)
 //   trans_a = 2:  C[M,N] = A[M,K]   * B[K,N]                 (input gradients)
 // 64x64x16 tiles, 256 threads, 4x4 register tile per thread.
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 

@@ -2,7 +2,7 @@
 // 75-joint FK passes (output and ground truth, anim/txform.py:10-34), 17 weighted L1 means (4 of them on frame-to-frame
 // differences) + the annealed KL term, /18 -- and the gradient of that scalar w.r.t. the decoder outputs.
 // One warp per frame, one tree level at a time; the kernels are described above loss_tree_kernel.
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 
@@ -584,13 +584,12 @@ __global__ void __launch_bounds__(LW_NP * 32) loss_w_final_kernel(const float* _
 
 struct LossWs { float *Dd, *fpartial, *F, *dq_own, *dq_prev; unsigned* S; TreeTables* tt; size_t bytes; };
 static LossWs loss_ws(void* base, int B, int T) {
-  LossWs w; size_t off = 0;
-  auto take = [&](size_t n) { float* p = base ? (float*)((char*)base + off) : nullptr; off += ((n * 4 + 255) / 256) * 256; return p; };
+  LossWs w; Arena a{(char*)base};
   const size_t BT = (size_t)B * T;
-  w.dq_own = take(BT * 4); w.dq_prev = take(BT * 4);
-  w.Dd = take(BT * LW_DD); w.fpartial = take(BT * LW_NP); w.tt = (TreeTables*)take(sizeof(TreeTables) / 4 + 1);
-  w.F = take(BT * NJ * 12); w.S = (unsigned*)take(BT * LW_SW);
-  w.bytes = off; return w;
+  w.dq_own = a.take(BT * 4); w.dq_prev = a.take(BT * 4);
+  w.Dd = a.take(BT * LW_DD); w.fpartial = a.take(BT * LW_NP); w.tt = (TreeTables*)a.take(sizeof(TreeTables) / 4 + 1);
+  w.F = a.take(BT * NJ * 12); w.S = (unsigned*)a.take(BT * LW_SW);
+  w.bytes = a.off; return w;
 }
 extern "C" size_t zeggs_loss_workspace_bytes(int B, int T) { return (B < 1 || T < 1) ? 0 : loss_ws(nullptr, B, T).bytes; }
 
@@ -609,12 +608,8 @@ extern "C" int zeggs_loss_fwd_bwd(const zeggs_loss_args* ap, void* stream_) {
   wa.Y[0] = a.Y; wa.Y[1] = a.WY; wa.rp[0] = a.root_pos; wa.rp[1] = a.W_root_pos; wa.rq[0] = a.root_rot; wa.rq[1] = a.W_root_rot;
   wa.gaze = a.gaze_pos; wa.tt = w.tt; wa.Dd = w.Dd; wa.partial = w.fpartial; wa.F = w.F; wa.S = w.S;
   wa.dY = a.dY; wa.dRootPos = a.dRootPos; wa.dq_own = w.dq_own; wa.dq_prev = w.dq_prev;
-  static bool attr = false;
-  if (!attr) {
-    ZCHECK_CUDA(cudaFuncSetAttribute(loss_w_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LW_WARPS * LW_FWD_FLOATS * sizeof(float))));
-    ZCHECK_CUDA(cudaFuncSetAttribute(loss_w_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LB_WARPS * 2 * LB_FRAME_FLOATS * sizeof(float))));
-    attr = true;
-  }
+  RC(set_max_dynamic_smem(loss_w_fwd_kernel, LW_WARPS * LW_FWD_FLOATS * sizeof(float)));
+  RC(set_max_dynamic_smem(loss_w_bwd_kernel, LB_WARPS * 2 * LB_FRAME_FLOATS * sizeof(float)));
   loss_tree_kernel<<<1, 96, 0, s>>>(a.parents, w.tt); count_launch();
   const int nb = ceil_div(BT, LW_WARPS);
   loss_w_fwd_kernel<<<nb, LW_WARPS * 32, LW_WARPS * LW_FWD_FLOATS * sizeof(float), s>>>(wa); count_launch();

@@ -9,7 +9,7 @@
 // the energy of its segment; a second kernel folds segments into blocks and applies the two gates.  Samples may be float32
 // or int16 PCM (x / 32768, audio_files.py:211-236).  The gain is applied by the mel kernel at load (mel.cu), not here:
 // the waveform is never rewritten in HBM.
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 

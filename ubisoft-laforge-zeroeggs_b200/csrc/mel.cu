@@ -5,7 +5,7 @@
 // written once).
 //
 // See mel_kernel below: register-resident 32 x 25 split of an 800-point complex FFT carrying two real frames.
-#include "decoder_common.cuh"
+#include "library.cuh"
 #include "mel_fft.cuh"
 
 namespace zeggs {
@@ -244,7 +244,7 @@ extern "C" int zeggs_mel_forward(const zeggs_mel_args* ap, void* stream_) {
   size_t smem = (size_t)(((nsamp_tile + 3) & ~3) + (MEL_FT + 2) * a.n_mels * (a.mel_out ? 2 : 1) + ((MEL_FT + 2 + 3) & ~3)) * sizeof(float)
               + (size_t)24 * 32 * sizeof(float2) + (size_t)MEL_WARPS * MEL_TB * sizeof(C2)
               + (size_t)((((a.fb_total > 0 && a.fb_total <= 4096 ? a.fb_total : 0) + 3) & ~3) + 3 * a.n_mels) * sizeof(float);
-  ZCHECK_CUDA(cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  RC(set_max_dynamic_smem(mel_kernel, smem));
   dim3 grid(ceil_div(L, MEL_FT), a.n_clips);
   ScopedTimer tm("mel", stream);
   mel_kernel<<<grid, MEL_WARPS * 32, smem, stream>>>(a, L, a.frames_per_anim);

@@ -3,7 +3,7 @@
 // ZEGGS/utils.py:47-87 (write_bvh: re-base the root on its first frame, apply start_position / start_rotation, fold the
 // root transform into joint 0), anim/quat.py:111-119 (to_euler 'zyx') and np.degrees.  One thread per (clip, frame, joint);
 // pure streaming: 36 B in, 24 B out per joint (+16 B when the local quaternions are requested).
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 

@@ -3,7 +3,7 @@
 // terms depend only on the step count and are evaluated on the host in double, as the reference does in
 // Python floats; `grad_scale` folds the 1/world_size of the data-parallel all-reduce into the same pass.
 #include <math.h>
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 

@@ -11,8 +11,7 @@
 // tau = row * L + column, row r holding outputs [32 L r, 32 L (r + 1)).  A CTA owns `nt` consecutive tasks, where nt is a
 // multiple of L (L <= 32: whole rows, i.e. 32 nt consecutive outputs) or a divisor of L (L > 32: part of one row); it stages
 // the decoded, mixed input span those outputs need in shared memory once.  Four partial sums per output, fp32.
-#include "common.cuh"
-#include "../../include/zeggs_b200.h"
+#include "library.cuh"
 
 namespace zeggs {
 void count_launch();
@@ -84,7 +83,7 @@ __global__ void __launch_bounds__(RS_THREADS) resample_kernel(const void* __rest
 template <int DT>
 int launch(const zeggs_resample_args& a, int nt, long long n_blocks, size_t smem, cudaStream_t s) {
   auto kern = resample_kernel<DT>;
-  if (smem > 48 * 1024) ZCHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (smem > 48 * 1024) RC(set_max_dynamic_smem(kern, smem));
   kern<<<(unsigned)n_blocks, RS_THREADS, smem, s>>>(a.pcm, a.n_in, a.channels, 1.0f / (float)a.channels, a.taps, a.L, a.M, a.K4,
                                                     a.delay, a.n_out, nt, a.out);
   count_launch();
@@ -113,12 +112,11 @@ extern "C" int zeggs_resample(const zeggs_resample_args* ap, void* stream_) {
   // every CTA's output range spans task_j0(nt - 1) + 31 L outputs (tau0 is aligned to nt, so no CTA crosses a row unevenly)
   const long long diff = task_j0(nt - 1, a.L) + 31LL * a.L;
   const long long span = diff * a.M / a.L + 2 + a.K4;
-  int dev = 0, smem_max = 0;
-  ZCHECK_CUDA(cudaGetDevice(&dev));
-  ZCHECK_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  DeviceLimits lim;
+  RC(device_limits(&lim));
   const size_t smem = (size_t)span * sizeof(float);
-  ZCHECK_SUPPORTED(smem <= (size_t)smem_max, "resample: L/M = %d/%d needs %zu bytes of shared memory per CTA (at most %d)", a.L, a.M, smem,
-                   smem_max);
+  ZCHECK_SUPPORTED(smem <= lim.smem_optin, "resample: L/M = %d/%d needs %zu bytes of shared memory per CTA (at most %zu)", a.L, a.M, smem,
+                   lim.smem_optin);
   ZCHECK_SUPPORTED(n_blocks < (1LL << 31), "resample: %lld output samples is too many", a.n_out);
   switch (a.dtype) {
     case ZEGGS_PCM_I16: return launch<ZEGGS_PCM_I16>(a, nt, n_blocks, smem, s);

@@ -18,7 +18,7 @@
 // The K dimension of each per-step product is staged through shared memory in 512-row chunks ([k][33] fp32, conflict-free for
 // 32 batch lanes; every thread has 8 global loads in flight per round, since the step is bound by the latency of this exchange);
 // batches larger than 32 loop over 32-sample tiles.
-#include "decoder_common.cuh"
+#include "library.cuh"
 
 namespace zeggs {
 
@@ -261,28 +261,14 @@ __global__ void rev_cell_bwd_kernel(int B, int H, const float* __restrict__ GIr,
 }
 
 // ------------------------------------------------------------------ host side
-template <typename K>
-static int launch_coop(K kern, int G, size_t smem, void** args, cudaStream_t s) {
-  ZCHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int dev = 0, nsm = 0, occ = 0;
-  ZCHECK_CUDA(cudaGetDevice(&dev));
-  ZCHECK_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  ZCHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GRU_THREADS, smem));
-  ZCHECK_ARG(occ * nsm >= G, "style GRU: cooperative grid of %d CTAs does not fit (%d SMs x %d)", G, nsm, occ);
-  ZCHECK_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(G), dim3(GRU_THREADS), args, smem, s));
-  count_launch();
-  return ZEGGS_OK;
-}
-
 int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
                          unsigned* bar, cudaStream_t s) {
   const int U = style_gru_units(H);
   ZCHECK_ARG(U > 0 && B >= 1 && T >= 1, "style GRU: hidden size %d unsupported (need H %% 4 == 0, H <= 528, or H %% 8 == 0, H <= 1056)", H);
   ZCHECK_CUDA(cudaMemsetAsync(bar, 0, 2 * sizeof(unsigned), s));
   ZCHECK_CUDA(cudaMemsetAsync(Hs, 0, (size_t)B * H * sizeof(float), s));     // h(-1) = 0
-  void* args[] = {(void*)&B, (void*)&T, (void*)&H, (void*)&Whh, (void*)&bhh, (void*)&GI, (void*)&Hs, (void*)&Gs, (void*)&hcat, (void*)&bar};
-  if (U == 4) return launch_coop(gru_fwd_kernel<4>, H / 4, gru_smem_bytes<4>(H, 0), args, s);
-  return launch_coop(gru_fwd_kernel<8>, H / 8, gru_smem_bytes<8>(H, 0), args, s);
+  if (U == 4) return launch_persistent(gru_fwd_kernel<4>, H / 4, GRU_THREADS, gru_smem_bytes<4>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
+  return launch_persistent(gru_fwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
 }
 
 int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs, const float* Gs, const float* dhf, int ld_dhf,
@@ -293,10 +279,9 @@ int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs,
              style_gru_max_batch(H), H);
   ZCHECK_CUDA(cudaMemsetAsync(bar, 0, 2 * sizeof(unsigned), s));
   const int nbt = (B + 31) / 32;
-  void* args[] = {(void*)&B, (void*)&T, (void*)&H, (void*)&Whh, (void*)&Hs, (void*)&Gs, (void*)&dhf, (void*)&ld_dhf, (void*)&dGih,
-                  (void*)&dGhh, (void*)&bar};
-  if (U == 4) return launch_coop(gru_bwd_kernel<4>, H / 4, gru_smem_bytes<4>(H, nbt), args, s);
-  return launch_coop(gru_bwd_kernel<8>, H / 8, gru_smem_bytes<8>(H, nbt), args, s);
+  if (U == 4)
+    return launch_persistent(gru_bwd_kernel<4>, H / 4, GRU_THREADS, gru_smem_bytes<4>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
+  return launch_persistent(gru_bwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
 }
 
 int style_gru_rev_cell_fwd(int B, int H, const float* GIr, const float* bhh, float* hcat, cudaStream_t s) {

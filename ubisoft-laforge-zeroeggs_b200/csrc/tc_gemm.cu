@@ -8,7 +8,7 @@
 // recovering ~fp32 product accuracy at 3x the tensor work.
 #include <cuda.h>
 #include <mutex>
-#include "decoder_common.cuh"
+#include "library.cuh"
 #include "tc_common.cuh"
 
 namespace zeggs {
@@ -311,16 +311,6 @@ static int encode_map(CUtensorMap* m, const void* base, int rows, int K, int ld_
   return ZEGGS_OK;
 }
 
-// SMs of the current device (one device per process: queried once)
-int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-  }
-  return n;
-}
-
 int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bfloat16* A_lo, int lda,
                    const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, const float* bias,
                    float* C, int ldc, int act, int accumulate, cudaStream_t stream, float* splitk_ws, size_t splitk_ws_bytes) {
@@ -342,19 +332,15 @@ int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bf
   }
   auto smem_of = [](int bm, int bn, int stages, int nop) { return (size_t)1024 + (size_t)stages * nop * (bm * TG_BK * 2 + bn * TG_BK * 2) + (2 * stages + 1) * 8 + 16; };
   const size_t smem = fused ? smem_of(128, 128, 3, 2) : BN == 256 ? smem_of(128, 256, 4, 1) : smem_of(128, 128, 4, 1);
-  static bool attr_set = false;     // one device per process (one rank per GPU): set once, not on every launch
-  if (!attr_set) {
-    ZCHECK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<128, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 128, 4, 1)));
-    ZCHECK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<256, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 256, 4, 1)));
-    ZCHECK_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<128, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(128, 128, 3, 2)));
-    attr_set = true;
-  }
+  RC(set_max_dynamic_smem(fused ? tc_gemm_kernel<128, 3, true> : BN == 128 ? tc_gemm_kernel<128, 4, false> : tc_gemm_kernel<256, 4, false>, smem));
+  DeviceLimits lim;
+  RC(device_limits(&lim));
   // split-K when the output has too few tiles to fill the SMs and the contraction is long: blockIdx.z writes its raw partial tile to
   // splitk_ws, and splitk_reduce_kernel sums them in a fixed order and applies the epilogue
   const int tiles = ceil_div(N, BN) * ceil_div(M, TG_BM), kblocks = ceil_div(K, TG_BK);
   int splits = 1;
-  if (splitk_ws && tiles <= num_sms() / 2 && kblocks >= 8) {
-    splits = std::min(std::max(1, num_sms() / tiles), kblocks / 2);
+  if (splitk_ws && tiles <= lim.sms / 2 && kblocks >= 8) {
+    splits = std::min(std::max(1, lim.sms / tiles), kblocks / 2);
     const size_t per = (size_t)M * N * sizeof(float);
     if ((size_t)splits * per > splitk_ws_bytes) splits = (int)(splitk_ws_bytes / per);
     splits = std::max(splits, 1);
@@ -385,7 +371,7 @@ int split_t_launch(const float* x, int rows, int cols, int ld_in, __nv_bfloat16*
 }
 
 // ------------------------------------------------------------------ fp32-in / fp32-out front end
-// The context of the entry point currently executing on this host thread (CtxScope in decoder_common.cuh): per-call state passed
+// The context of the entry point currently executing on this host thread (CtxScope in library.cuh): per-call state passed
 // by the caller.  Calls that pass none get k_no_ctx: no scratch, so products run on the fp32 SIMT kernel and convolutions take the
 // im2col path.
 static const zeggs_ctx k_no_ctx = {nullptr, 0, 1, 0};
@@ -421,19 +407,17 @@ static int plan_tc_operands(int rows_a, int rows_b, int Kp, double macs, bool wg
   const zeggs_ctx& c = *tl_ctx;
   ZCHECK_ARG(c.gemm_mode == 0 || c.gemm_mode == 1, "zeggs_ctx.gemm_mode must be 0 (fp32 SIMT) or 1 (tensor-core split-bf16), got %d",
              c.gemm_mode);
-  char* const base = (char*)c.scratch;
-  if (c.gemm_mode == 0 || base == nullptr || macs < 4.0e6) return ZEGGS_CONV_NOT_TAKEN;
+  if (c.gemm_mode == 0 || c.scratch == nullptr || macs < 4.0e6) return ZEGGS_CONV_NOT_TAKEN;
   const bool lo = !(wgrad && c.fast_wgrad);
-  char* p = base;
-  auto take = [&](int rows) { __nv_bfloat16* r = (__nv_bfloat16*)p; p += ((size_t)rows * Kp * 2 + 255) / 256 * 256; return r; };
-  op->Ah = take(rows_a);
-  op->Bh = take(rows_b);
-  op->Al = lo ? take(rows_a) : nullptr;
-  op->Bl = lo ? take(rows_b) : nullptr;
-  p = (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255);
-  if ((size_t)(p - base) > c.scratch_bytes) return ZEGGS_CONV_NOT_TAKEN;
-  op->ws = (float*)p;
-  op->ws_bytes = c.scratch_bytes - (size_t)(p - base);
+  Arena a{(char*)c.scratch};
+  op->Ah = (__nv_bfloat16*)a.bytes((size_t)rows_a * Kp * 2);
+  op->Bh = (__nv_bfloat16*)a.bytes((size_t)rows_b * Kp * 2);
+  op->Al = lo ? (__nv_bfloat16*)a.bytes((size_t)rows_a * Kp * 2) : nullptr;
+  op->Bl = lo ? (__nv_bfloat16*)a.bytes((size_t)rows_b * Kp * 2) : nullptr;
+  a.align(256);
+  if (a.off > c.scratch_bytes) return ZEGGS_CONV_NOT_TAKEN;
+  op->ws = (float*)a.here();
+  op->ws_bytes = a.rest(c.scratch_bytes);
   return ZEGGS_OK;
 }
 
@@ -541,7 +525,9 @@ int conv_gemm_fwd(const float* x, int B, int T, int C, int k, int pad, int repli
   TcOperands op;
   const int rc = plan_tc_operands(M, N, Kp, (double)M * N * K, false, &op);
   if (rc) return rc;
-  im2col_split_kernel<<<std::min(M, num_sms() * 16), 256, 0, stream>>>(x, B, T, C, k, pad, replicate, op.Ah, op.Al, Kp);
+  DeviceLimits lim;
+  RC(device_limits(&lim));
+  im2col_split_kernel<<<std::min(M, lim.sms * 16), 256, 0, stream>>>(x, B, T, C, k, pad, replicate, op.Ah, op.Al, Kp);
   count_launch();
   split_bf16_kernel<<<592, 256, 0, stream>>>(W, N, K, K, op.Bh, op.Bl, Kp);
   count_launch();
