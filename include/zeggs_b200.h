@@ -320,24 +320,6 @@ int zeggs_style_enc_gru_fwd(const zeggs_style_enc_gru_args* a, void* stream);
 int zeggs_style_enc_gru_bwd(const zeggs_style_enc_gru_args* a, const zeggs_style_enc_gru_grads* g, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * One teacher-forced decoder step (RecurrentDecoderNormal.forward, modules.py:179-185), fp32 throughout:
- *   pose [B,1134] (the normalised input vector of modules.py:699-713), speech [B,S], style [B,Z], h_in [2,B,H]
- *   -> y [B,1131] (normalised output of layer2), h_out [2,B,H].
- * The tight parity point (<= 1e-4 vs the reference per step) and the unit of streaming inference; windows go through
- * zeggs_decoder_window_fwd.
- */
-typedef struct {
-  int B, H, S, Z;
-  const float *W0, *b0, *W_ih0, *b_ih0, *W_hh0, *b_hh0, *W_ih1, *b_ih1, *W_hh1, *b_hh1, *W2, *b2;
-  const float *pose, *speech, *style, *h_in;
-  float *y, *h_out;
-  void* workspace;
-  size_t workspace_bytes;
-} zeggs_decoder_step_args;
-size_t zeggs_decoder_step_workspace_bytes(int B, int H, int S, int Z);
-int zeggs_decoder_step_fwd(const zeggs_decoder_step_args* a, void* stream);
-
-/* ------------------------------------------------------------------------------------------------
  * Training loss, forward and backward in one call (train.py:277-421): world-space transforms, 75-joint FK with
  * velocities for the output and the ground truth, 17 weighted L1 means + kl_weight * KL(mu, logvar), divided by 18.
  * (Y, root_pos, root_rot) are the decoder outputs; (WY, W_root_pos, W_root_rot) the ground-truth window in the
@@ -405,11 +387,8 @@ int zeggs_window_gather(const zeggs_gather_args* a, void* stream);
 /* Input normalisation of train.py:232-234 / 247-249 in one pass: out[r][c] = (x[r][c] - mean[c]) / std[c]  (x, out: [rows][C] fp32). */
 int zeggs_normalize_rows(const float* x, const float* mean, const float* stdv, float* out, long long rows, int C, void* stream);
 
-/* Fused RAdam step over a flat fp32 parameter buffer (optimizers.py:31-99; weight_decay 0,
- * degenerated_to_sgd).  `step` is the 1-based step count; gradients are multiplied by grad_scale first. */
-int zeggs_radam_step(float* p, const float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2,
-                     float eps, int step, float grad_scale, void* stream);
-/* The same step with every step-dependent scalar in DEVICE memory, so that a captured CUDA graph can be replayed:
+/* Fused RAdam step over a flat fp32 parameter buffer (optimizers.py:31-99; weight_decay 0, degenerated_to_sgd), with every
+ * step-dependent scalar in DEVICE memory, so that a captured CUDA graph can be replayed (gradients are multiplied by grad_scale first):
  * hyper[0..4] = lr, beta1, beta2, eps, grad_scale (inputs; the host rewrites them between replays when they change),
  * hyper[5..7] = scratch written by the call; *step_count is the number of steps taken so far and is incremented by the call
  * (the rectification terms of optimizers.py:66-78 are evaluated on the device in double from *step_count + 1). */

@@ -225,13 +225,13 @@ def test_splitk_workspace_at_the_end_of_the_scratch(dev, ops, private_lane):
 
 # ---------------------------------------------------------------------------------------------------------- batch limit
 def _fwd_smem(U, nbt):
-    """launch_fwd (csrc/decoder_fwd.cu): dynamic shared memory of the forward recurrence."""
+    """fwd_smem_bytes (csrc/decoder_fwd.cu): dynamic shared memory of the forward recurrence."""
     stg = 16 * 4 * (6 * U // 4) + 1024
     return (8 * 2 * stg + 8 * 6 * U * 32 + nbt * 3 * U * 32 + 6 * 32) * 4
 
 
 def _bwd_smem(H, U, nbt):
-    """launch_bwd (csrc/decoder_bwd.cu): dynamic shared memory of the BPTT recurrence."""
+    """bwd_smem_bytes (csrc/decoder_bwd.cu): dynamic shared memory of the BPTT recurrence."""
     n4b = math.ceil(max(9, math.ceil(1134 / (H // U))) / 16)
     stg = 16 * 16 + 1024
     return (8 * 2 * stg + 8 * 16 * 32 + 2 * nbt * U * 32 + nbt * n4b * 16 * 32 + nbt * 9 * 32 + nbt * 7 * 32) * 4

@@ -75,7 +75,7 @@ def test_film_wide(dev, ops, H, B, T):
 
 
 def _fwd_smem_u16(nbt):
-    """launch_fwd at U = 16: the stage buffers and reduction tile of one 8-unit pass, gi0p for all 16 units of each batch tile."""
+    """fwd_smem_bytes<16> (csrc/decoder_fwd.cu): the stage buffers and reduction tile of one 8-unit pass, gi0p for all 16 units of each batch tile."""
     stg = 16 * 48 + 1024
     return (8 * 2 * stg + 8 * 48 * 32 + nbt * 3 * 16 * 32 + 6 * 32) * 4
 

@@ -98,10 +98,6 @@ StyleEncGruArgs = _struct("StyleEncGruArgs", ints=("B", "T", "C_in", "H", "E"), 
 StyleEncGruGrads = _struct("StyleEncGruGrads", ptrs=("dz", "dmu", "dlogvar") + tuple("d" + n for n in STYLE_GRU_W))
 
 
-DecoderStepArgs = _struct("DecoderStepArgs", ints=("B", "H", "S", "Z"),
-                          ptrs=("W0", "b0", "W_ih0", "b_ih0", "W_hh0", "b_hh0", "W_ih1", "b_ih1", "W_hh1", "b_hh1", "W2", "b2",
-                                "pose", "speech", "style", "h_in", "y", "h_out", "workspace"),
-                          tail=[("workspace_bytes", C.c_size_t)])
 LossArgs = _struct("LossArgs", ints=("B", "T", "Z"), floats=("dt", "kl_weight"),
                    ptrs=("Y", "root_pos", "root_rot", "WY", "W_root_pos", "W_root_rot", "gaze_pos", "parents", "mu", "logvar",
                          "losses", "dY", "dRootPos", "dRootRot", "dmu", "dlogvar", "workspace"),
@@ -129,7 +125,7 @@ ResampleArgs = _struct("ResampleArgs", tail=[("n_in", C.c_longlong), ("n_out", C
 def struct_mirrors():
     return {"zeggs_ctx": Ctx, "zeggs_mel_args": MelArgs, "zeggs_loudness_args": LoudnessArgs, "zeggs_decoder_fwd_args": DecoderFwdArgs,
             "zeggs_decoder_bwd_args": DecoderBwdArgs, "zeggs_speech_enc_args": SpeechEncArgs, "zeggs_speech_enc_grads": SpeechEncGrads,
-            "zeggs_style_enc_args": StyleEncArgs, "zeggs_style_enc_grads": StyleEncGrads, "zeggs_decoder_step_args": DecoderStepArgs,
+            "zeggs_style_enc_args": StyleEncArgs, "zeggs_style_enc_grads": StyleEncGrads,
             "zeggs_loss_args": LossArgs, "zeggs_pose_post_args": PosePostArgs, "zeggs_gather_args": GatherArgs,
             "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads,
             "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs,
@@ -147,8 +143,6 @@ SYMBOLS = [
     ("zeggs_timing_read", C.c_int, [C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_int)]),
     ("zeggs_mel_num_frames", C.c_int, [C.c_int, C.c_int, C.c_int]),
     ("zeggs_mel_forward", C.c_int, [C.POINTER(MelArgs), C.c_void_p]),
-    ("zeggs_decoder_step_workspace_bytes", C.c_size_t, [C.c_int] * 4),
-    ("zeggs_decoder_step_fwd", C.c_int, [C.POINTER(DecoderStepArgs), C.c_void_p]),
     ("zeggs_window_gather", C.c_int, [C.POINTER(GatherArgs), C.c_void_p]),
     ("zeggs_normalize_rows", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
     ("zeggs_pose_to_bvh_channels", C.c_int, [C.POINTER(PosePostArgs), C.c_void_p]),
@@ -192,7 +186,6 @@ SYMBOLS = [
     ("zeggs_dropout_mask_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_float, C.c_void_p, C.c_ulonglong, C.c_void_p]),
     ("zeggs_randn_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_ulonglong, C.c_void_p]),
     ("zeggs_radam_step_dev", C.c_int, [C.c_void_p] * 4 + [C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
-    ("zeggs_radam_step", C.c_int, [C.c_void_p] * 4 + [C.c_size_t, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_float, C.c_void_p]),
     ("zeggs_sgemm", C.c_int, [C.c_int] * 4 + [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                C.c_int, C.c_int, C.c_int, C.c_void_p]),
     ("zeggs_tc_gemm_bf16", C.c_int, [C.c_int] * 3 + [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,

@@ -150,7 +150,7 @@ extern "C" int zeggs_timing_read(const char* name, double* total_ms, int* count)
 }
 
 extern "C" const char* zeggs_last_error(void) { return zeggs::get_error(); }
-extern "C" int zeggs_version(void) { return 102; }
+extern "C" int zeggs_version(void) { return 103; }
 extern "C" long long zeggs_launch_count(void) { return zeggs::g_launches.load(); }
 
 // sizeof of every args struct of include/zeggs_b200.h by its C name (0 = unknown): lets a binding in another language check at load
@@ -159,7 +159,7 @@ extern "C" size_t zeggs_struct_size(const char* name) {
   if (!name) return 0;
 #define ZS(T) if (!strcmp(name, #T)) return sizeof(T);
   ZS(zeggs_ctx) ZS(zeggs_mel_args) ZS(zeggs_loudness_args) ZS(zeggs_decoder_fwd_args) ZS(zeggs_decoder_bwd_args) ZS(zeggs_speech_enc_args)
-  ZS(zeggs_speech_enc_grads) ZS(zeggs_style_enc_args) ZS(zeggs_style_enc_grads) ZS(zeggs_decoder_step_args) ZS(zeggs_loss_args)
+  ZS(zeggs_speech_enc_grads) ZS(zeggs_style_enc_args) ZS(zeggs_style_enc_grads) ZS(zeggs_loss_args)
   ZS(zeggs_pose_post_args) ZS(zeggs_gather_args) ZS(zeggs_style_enc_gru_args) ZS(zeggs_style_enc_gru_grads)
   ZS(zeggs_anim_features_args) ZS(zeggs_spline_args) ZS(zeggs_moments_args) ZS(zeggs_resample_args)
   ZS(zeggs_decoder_film_fwd_args) ZS(zeggs_decoder_film_bwd_args)

@@ -146,7 +146,6 @@ __host__ __device__ inline V3 quat_from_helical_bwd(V3 h, Q4 dE) {
 }
 
 __device__ __forceinline__ float elu_f(float x) { return x > 0.0f ? x : expm1f(x); }
-__device__ __forceinline__ float elu_grad_from_pre(float pre) { return pre > 0.0f ? 1.0f : expf(pre); }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // ------------------------------------------------------------------ async copy / cache-controlled access
@@ -159,7 +158,6 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 __device__ __forceinline__ float ld_cg(const float* p) { return __ldcg(p); }
-__device__ __forceinline__ float4 ld_cg4(const float4* p) { return __ldcg(p); }
 
 // ------------------------------------------------------------------ grid-wide barrier for persistent kernels
 // All CTAs of a cooperative launch call grid_sync() the same number of times.  `bar` points at two

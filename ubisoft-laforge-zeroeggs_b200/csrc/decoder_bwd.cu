@@ -489,15 +489,17 @@ extern "C" size_t zeggs_decoder_packed_bwd_bytes(int H, int S, int Z) {
   return make_bgeom(g).total * sizeof(float);
 }
 
-extern "C" int zeggs_decoder_pack_weights_bwd(const zeggs_decoder_fwd_args* a, float* packed, void* stream_) {
+// the transposed slices of geometry g: the whole pack of the normal decoder, the front of the FiLM decoder's
+static int pack_bwd_slices(const zeggs_decoder_fwd_args& a, const DecGeom& g, float* packed, cudaStream_t stream) {
+  pack_decoder_bwd_kernel<<<592, 256, 0, stream>>>(g, make_bgeom(g), a.W0, a.W_ih0, a.W_hh0, a.W_ih1, a.W_hh1, a.W2, packed);
+  LAUNCH_OK();
+  return ZEGGS_OK;
+}
+
+extern "C" int zeggs_decoder_pack_weights_bwd(const zeggs_decoder_fwd_args* a, float* packed, void* stream) {
   CtxScope ctx_scope(a ? a->ctx : nullptr);
   ZCHECK_ARG(a && packed && fp32_hidden_ok(a->H), "decoder bwd pack: bad arguments");
-  DecGeom g = make_geom(a->B, a->H, a->S, a->Z);
-  BwdGeom bg = make_bgeom(g);
-  pack_decoder_bwd_kernel<<<592, 256, 0, (cudaStream_t)stream_>>>(g, bg, a->W0, a->W_ih0, a->W_hh0, a->W_ih1, a->W_hh1, a->W2, packed);
-  count_launch();
-  ZCHECK_LAUNCH();
-  return ZEGGS_OK;
+  return pack_bwd_slices(*a, make_geom(a->B, a->H, a->S, a->Z), packed, (cudaStream_t)stream);
 }
 
 extern "C" size_t zeggs_decoder_bwd_workspace_bytes(int B, int T, int H, int S, int Z) {
@@ -512,7 +514,6 @@ static size_t bwd_smem_bytes(const DecGeom& g, const BwdGeom& bg, int nbt) {
          sizeof(float);
 }
 
-// the fp32 backward, normal and FiLM, refuses a batch its shared memory cannot hold before it enqueues anything
 static int check_bwd_batch(const DecGeom& g, const BwdGeom& bg) {
   DeviceLimits lim;
   RC(device_limits(&lim));
@@ -522,10 +523,21 @@ static int check_bwd_batch(const DecGeom& g, const BwdGeom& bg) {
   return ZEGGS_OK;
 }
 
-template <int U, bool FILM>
-static int launch_bwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const BwdGeom& bg, const DecWs& w, const BwdWs& bw,
-                      const BwdArgsDev& d, const FilmDev& f, cudaStream_t stream) {
-  return launch_persistent(decoder_bwd_kernel<U, FILM>, g.G, 256, bwd_smem_bytes(g, bg, g.nbt), 1, stream, a, g, bg, w, bw, d, f);
+// the BPTT recurrence of the fp32 engine, normal and FiLM.  It refuses a batch its shared memory cannot hold before it enqueues anything.
+template <bool FILM>
+static int bptt_fp32(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& b, const DecGeom& g, const DecWs& w, const BwdWs& bw,
+                     const FilmDev& f, cudaStream_t stream) {
+  const BwdGeom bg = make_bgeom(g);
+  RC(check_bwd_batch(g, bg));
+  ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
+  ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)a.T * g.nbt * K1P * 32 * sizeof(float), stream));
+  // the FiLM recurrence writes the rows t >= 1 of DGB; the rows t = 0 stay zero
+  if constexpr (FILM) ZCHECK_CUDA(cudaMemsetAsync(f.DGB, 0, (size_t)a.B * a.T * 4 * a.H * sizeof(float), stream));
+  BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
+  ScopedTimer tm("decoder_bwd", stream);
+  return dispatch_units(g.U, [&](auto u) {
+    return launch_persistent(decoder_bwd_kernel<u, FILM>, g.G, 256, bwd_smem_bytes(g, bg, g.nbt), 1, stream, a, g, bg, w, bw, d, f);
+  });
 }
 
 static int wgrad(const float* GA, long long gaT, long long gaBT, int N, const float* XB, long long xbT, long long xbBT, int K,
@@ -676,20 +688,8 @@ static int decoder_window_bwd_fp32(const zeggs_decoder_fwd_args& a, const zeggs_
                                    const BwdWs& bw, cudaStream_t stream) {
   ZCHECK_ARG(b.packed_bwd, "decoder bwd: packed_bwd missing");
   if (b.phase == 2) return ZEGGS_OK;
-  const int T = a.T, nbt = g.nbt;
-  const BwdGeom bg = make_bgeom(g);
   int rc;
-  RC(check_bwd_batch(g, bg));
-  ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
-  ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
-  {
-    BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
-    ScopedTimer tm("decoder_bwd", stream);
-    const FilmDev none = {};
-    rc = g.U == 4 ? launch_bwd<4, false>(a, g, bg, w, bw, d, none, stream)
-       : g.U == 8 ? launch_bwd<8, false>(a, g, bg, w, bw, d, none, stream) : launch_bwd<16, false>(a, g, bg, w, bw, d, none, stream);
-    if (rc) return rc;
-  }
+  if ((rc = bptt_fp32<false>(a, b, g, w, bw, FilmDev{}, stream))) return rc;
   ScopedTimer tm("decoder_wgrad", stream);
   if ((rc = cond_kmajor(a, g, bw, stream))) return rc;
   // weight gradients: tensor-core GEMMs over split-bf16 copies of the histories when those fit the scratch buffer (a second, lo pass
@@ -783,11 +783,9 @@ extern "C" int zeggs_decoder_pack_weights_bwd_film(const zeggs_decoder_film_fwd_
   DecGeom g = make_film_geom(a.B, a.H, a.S, a.Z);
   BwdGeom bg = make_bgeom(g);
   cudaStream_t stream = (cudaStream_t)stream_;
-  pack_decoder_bwd_kernel<<<592, 256, 0, stream>>>(g, bg, a.W0, a.W_ih0, a.W_hh0, a.W_ih1, a.W_hh1, a.W2, packed);
-  count_launch();
+  int rc = pack_bwd_slices(a, g, packed, stream); if (rc) return rc;
   pack_film_bwd_kernel<<<264, 256, 0, stream>>>(g, bg.R1, f->Wm, packed + bg.total);
-  count_launch();
-  ZCHECK_LAUNCH();
+  LAUNCH_OK();
   return ZEGGS_OK;
 }
 
@@ -834,19 +832,8 @@ extern "C" int zeggs_decoder_film_window_bwd(const zeggs_decoder_film_fwd_args* 
   ZCHECK_ARG(a.workspace_bytes >= fwd_bytes, "film decoder bwd: forward workspace too small (%zu < %zu)", a.workspace_bytes, fwd_bytes);
   ZCHECK_ARG(b.workspace && b.workspace_bytes >= need, "film decoder bwd: workspace too small (%zu < %zu)", b.workspace_bytes, need);
   const int nbt = g.nbt, BT = a.B * T;
-  const BwdGeom bg = make_bgeom(g);
   int rc;
-  RC(check_bwd_batch(g, bg));
-  ZCHECK_CUDA(cudaMemsetAsync(bw.bar, 0, 256, stream));
-  ZCHECK_CUDA(cudaMemsetAsync(bw.DY, 0, (size_t)T * nbt * K1P * 32 * sizeof(float), stream));
-  ZCHECK_CUDA(cudaMemsetAsync(f.DGB, 0, (size_t)BT * 4 * H * sizeof(float), stream));
-  {
-    BwdArgsDev d; d.dY = b.dY; d.dRootPos = b.dRootPos; d.dRootRot = b.dRootRot; d.packed = b.packed_bwd;
-    ScopedTimer tm("decoder_bwd", stream);
-    rc = g.U == 4 ? launch_bwd<4, true>(a, g, bg, w, bw, d, f, stream)
-       : g.U == 8 ? launch_bwd<8, true>(a, g, bg, w, bw, d, f, stream) : launch_bwd<16, true>(a, g, bg, w, bw, d, f, stream);
-    if (rc) return rc;
-  }
+  if ((rc = bptt_fp32<true>(a, b, g, w, bw, f, stream))) return rc;
   ScopedTimer tm("decoder_wgrad", stream);
   // the recurrence's conditioning input is the speech alone: the normal decoder's host steps with no style columns
   zeggs_decoder_fwd_args as = a;

@@ -1,6 +1,7 @@
 // Geometry, workspace layout and the weight-stationary "skinny GEMM" building block shared by the
 // decoder forward and backward persistent kernels.
 #pragma once
+#include <type_traits>
 #include "library.cuh"
 
 namespace zeggs {
@@ -14,6 +15,15 @@ inline int pick_U(int H) {
   if (H % 8 == 0 && H / 8 <= 132) return 8;
   if (H % 16 == 0 && H / 16 <= 132) return 16;
   return -1;
+}
+
+// calls f(std::integral_constant<int, U>{}) for the units per CTA pick_U chose (4, 8 or 16): the one place a run-time U becomes the
+// template argument of the fp32 kernels
+template <class F>
+auto dispatch_units(int U, F&& f) {
+  if (U == 4) return f(std::integral_constant<int, 4>{});
+  if (U == 8) return f(std::integral_constant<int, 8>{});
+  return f(std::integral_constant<int, 16>{});
 }
 
 // units of one pass of the fp32 recurrences: a CTA's U units are U / pass_units(U) passes, each with its own contiguous weight slice

@@ -348,7 +348,7 @@ static int check_fwd_args(const zeggs_decoder_fwd_args* a) {
   ZCHECK_ARG(a->S >= 1 && a->Z >= 1 && a->S + a->Z <= 256, "decoder: bad S=%d Z=%d", a->S, a->Z);
   if (a->engine != 1) {
     const int U = pick_U(a->H);
-    size_t (*smem_of)(int) = U == 4 ? fwd_smem_bytes<4> : U == 8 ? fwd_smem_bytes<8> : fwd_smem_bytes<16>;
+    auto smem_of = [U](int nbt) { return dispatch_units(U, [nbt](auto u) { return fwd_smem_bytes<u>(nbt); }); };
     const int nbt = ceil_div(a->B, 32);
     DeviceLimits lim;
     RC(device_limits(&lim));
@@ -364,15 +364,17 @@ extern "C" size_t zeggs_decoder_packed_bytes(int H, int S, int Z) {
   return g.packed_floats() * sizeof(float);
 }
 
-extern "C" int zeggs_decoder_pack_weights(const zeggs_decoder_fwd_args* a, float* packed, void* stream_) {
+// P1-P4 of geometry g: the whole pack of the normal decoder, the front of the FiLM decoder's
+static int pack_fwd_slices(const zeggs_decoder_fwd_args& a, const DecGeom& g, float* packed, cudaStream_t stream) {
+  pack_decoder_kernel<<<592, 256, 0, stream>>>(g, a.W0, a.W_ih0, a.W_hh0, a.W_ih1, a.W_hh1, a.W2, packed);
+  LAUNCH_OK();
+  return ZEGGS_OK;
+}
+
+extern "C" int zeggs_decoder_pack_weights(const zeggs_decoder_fwd_args* a, float* packed, void* stream) {
   CtxScope ctx_scope(a ? a->ctx : nullptr);
   int rc = check_fwd_args(a); if (rc) return rc;
-  cudaStream_t stream = (cudaStream_t)stream_;
-  DecGeom g = make_geom(a->B, a->H, a->S, a->Z);
-  pack_decoder_kernel<<<592, 256, 0, stream>>>(g, a->W0, a->W_ih0, a->W_hh0, a->W_ih1, a->W_hh1, a->W2, packed);
-  count_launch();
-  ZCHECK_LAUNCH();
-  return ZEGGS_OK;
+  return pack_fwd_slices(*a, make_geom(a->B, a->H, a->S, a->Z), packed, (cudaStream_t)stream);
 }
 
 extern "C" size_t zeggs_decoder_workspace_bytes(int B, int T, int H, int S, int Z, int save) {
@@ -381,14 +383,10 @@ extern "C" size_t zeggs_decoder_workspace_bytes(int B, int T, int H, int S, int 
   return make_ws(nullptr, g, T, save).bytes;
 }
 
-template <int U, bool FILM>
-static int launch_fwd(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, const FilmDev& f, cudaStream_t stream) {
-  // the shared memory is within the device's limit: check_fwd_args
-  return launch_persistent(decoder_fwd_kernel<U, FILM>, g.G, 256, fwd_smem_bytes<U>(g.nbt), 1, stream, a, g, w, f);
-}
-
-// fp32 engine: the hoisted speech / style terms, then the SIMT recurrence
-static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, cudaStream_t stream) {
+// fp32 engine, normal and FiLM: the hoisted conditioning terms of `a` (the FiLM decoder passes Z = 0: its recurrence reads the speech
+// alone), then the SIMT recurrence
+template <bool FILM>
+static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& g, const DecWs& w, const FilmDev& f, cudaStream_t stream) {
   const int C = a.S + a.Z;
   const size_t sm = (size_t)(C * 33 + 64 * (C + 1)) * sizeof(float);
   RC(set_max_dynamic_smem(cond_precompute_kernel, sm));
@@ -396,9 +394,10 @@ static int decoder_fwd_fp32_run(const zeggs_decoder_fwd_args& a, const DecGeom& 
   count_launch();
   ZCHECK_LAUNCH();
   ScopedTimer tm("decoder_fwd", stream);
-  const FilmDev none = {};
-  if (g.U == 16) return launch_fwd<16, false>(a, g, w, none, stream);
-  return g.U == 4 ? launch_fwd<4, false>(a, g, w, none, stream) : launch_fwd<8, false>(a, g, w, none, stream);
+  // the shared memory is within the device's limit: check_fwd_args
+  return dispatch_units(g.U, [&](auto u) {
+    return launch_persistent(decoder_fwd_kernel<u, FILM>, g.G, 256, fwd_smem_bytes<u>(g.nbt), 1, stream, a, g, w, f);
+  });
 }
 
 // frame 0 and the initial GRU state (modules.py:72-98), shared by both decoders
@@ -434,7 +433,7 @@ extern "C" int zeggs_decoder_window_fwd(const zeggs_decoder_fwd_args* ap, void* 
   ZCHECK_SUPPORTED(a.engine != 1 || tc_hidden_ok(a.H), "decoder tc engine: hidden size %d unsupported (needs H %% 128 == 0, 384 <= H <= 1024)", a.H);
   if ((rc = decoder_fwd_prologue(a, g, w, stream))) return rc;
   if (a.T == 1) return ZEGGS_OK;
-  return a.engine == 1 ? decoder_fwd_tc_run(a, g, w, stream) : decoder_fwd_fp32_run(a, g, w, stream);
+  return a.engine == 1 ? decoder_fwd_tc_run(a, g, w, stream) : decoder_fwd_fp32_run<false>(a, g, w, FilmDev{}, stream);
 }
 
 // ------------------------------------------------------------------ FiLM decoder (fp32 engine)
@@ -470,11 +469,9 @@ extern "C" int zeggs_decoder_pack_weights_film(const zeggs_decoder_film_fwd_args
   const zeggs_decoder_fwd_args& a = f->dec;
   cudaStream_t stream = (cudaStream_t)stream_;
   DecGeom g = make_film_geom(a.B, a.H, a.S, a.Z);
-  pack_decoder_kernel<<<592, 256, 0, stream>>>(g, a.W0, a.W_ih0, a.W_hh0, a.W_ih1, a.W_hh1, a.W2, packed);
-  count_launch();
+  if ((rc = pack_fwd_slices(a, g, packed, stream))) return rc;
   pack_film_kernel<<<264, 256, 0, stream>>>(g, f->Wm, packed + g.packed_floats());
-  count_launch();
-  ZCHECK_LAUNCH();
+  LAUNCH_OK();
   return ZEGGS_OK;
 }
 
@@ -504,17 +501,10 @@ extern "C" int zeggs_decoder_film_window_fwd(const zeggs_decoder_film_fwd_args* 
   float* GB = const_cast<float*>(f.GB);
   rc = gemm_f32_auto(0, a.B * a.T, 2 * a.H, a.Z, a.style, a.Z, fp->Wg, a.Z, fp->bg, GB, 4 * a.H, 0, 0, stream); if (rc) return rc;
   rc = gemm_f32_auto(0, a.B * a.T, 2 * a.H, a.Z, a.style, a.Z, fp->Wb, a.Z, fp->bb, GB + 2 * a.H, 4 * a.H, 0, 0, stream); if (rc) return rc;
-  // the speech columns of layer0 / GRU0 hoisted out of the recurrence: the normal decoder's pre-pass with no style columns
+  // style does not enter layer0 / GRU0: the normal decoder's pre-pass and recurrence with no style columns
   zeggs_decoder_fwd_args as = a;
   as.Z = 0;
-  const size_t sm = (size_t)(a.S * 33 + 64 * (a.S + 1)) * sizeof(float);
-  RC(set_max_dynamic_smem(cond_precompute_kernel, sm));
-  cond_precompute_kernel<<<dim3(a.T, g.nbt, ceil_div(4 * a.H, 64)), 256, sm, stream>>>(as, g, w.S01);
-  count_launch();
-  ZCHECK_LAUNCH();
-  ScopedTimer tm("decoder_fwd", stream);
-  if (g.U == 16) return launch_fwd<16, true>(a, g, w, f, stream);
-  return g.U == 4 ? launch_fwd<4, true>(a, g, w, f, stream) : launch_fwd<8, true>(a, g, w, f, stream);
+  return decoder_fwd_fp32_run<true>(as, g, w, f, stream);
 }
 
 }  // namespace zeggs

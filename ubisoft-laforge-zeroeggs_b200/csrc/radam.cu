@@ -1,26 +1,13 @@
 // Fused multi-tensor RAdam (ZEGGS/optimizers.py:31-99) over one flat fp32 parameter buffer:
-// weight_decay = 0, degenerated_to_sgd = True (the configuration train.py:160 uses).  The rectification
-// terms depend only on the step count and are evaluated on the host in double, as the reference does in
-// Python floats; `grad_scale` folds the 1/world_size of the data-parallel all-reduce into the same pass.
+// weight_decay = 0, degenerated_to_sgd = True (the configuration train.py:160 uses).  The step count and the
+// hyper-parameters live in device memory, so a captured CUDA graph can replay the step.  The rectification terms
+// depend only on the step count; one thread evaluates them in double, as the reference does in Python floats, and
+// the main kernel reads them back.  `grad_scale` folds the 1/world_size of the data-parallel all-reduce into the same pass.
 #include <math.h>
 #include "library.cuh"
 
 namespace zeggs {
 
-__global__ void radam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                             size_t n, float beta1, float beta2, float eps, float step_lr, int adaptive, float grad_scale) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float gi = g[i] * grad_scale;
-    const float vi = v[i] * beta2 + (1.0f - beta2) * gi * gi;     // optimizers.py:58
-    const float mi = m[i] * beta1 + (1.0f - beta1) * gi;          // :59
-    v[i] = vi; m[i] = mi;
-    if (adaptive) p[i] = p[i] - step_lr * mi / (sqrtf(vi) + eps); // :88-89
-    else p[i] = p[i] - step_lr * mi;                              // :94
-  }
-}
-
-// device-resident variant (CUDA-graph replay): the step count lives in device memory; one thread evaluates the rectification
-// terms in double exactly as the host path does, the main kernel reads them back
 __global__ void radam_prep_kernel(float* __restrict__ hyper, int* __restrict__ step_count) {
   const int step = *step_count + 1;
   *step_count = step;
@@ -46,11 +33,11 @@ __global__ void radam_dev_kernel(float* __restrict__ p, const float* __restrict_
   const bool adaptive = hyper[6] != 0.f;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const float gi = g[i] * grad_scale;
-    const float vi = v[i] * beta2 + (1.0f - beta2) * gi * gi;
-    const float mi = m[i] * beta1 + (1.0f - beta1) * gi;
+    const float vi = v[i] * beta2 + (1.0f - beta2) * gi * gi;     // optimizers.py:58
+    const float mi = m[i] * beta1 + (1.0f - beta1) * gi;          // :59
     v[i] = vi; m[i] = mi;
-    if (adaptive) p[i] = p[i] - step_lr * mi / (sqrtf(vi) + eps);
-    else p[i] = p[i] - step_lr * mi;
+    if (adaptive) p[i] = p[i] - step_lr * mi / (sqrtf(vi) + eps); // :88-89
+    else p[i] = p[i] - step_lr * mi;                              // :94
   }
 }
 extern "C" int zeggs_radam_step_dev(float* p, const float* g, float* m, float* v, size_t n, float* hyper, int* step_count, void* stream) {
@@ -61,31 +48,6 @@ extern "C" int zeggs_radam_step_dev(float* p, const float* g, float* m, float* v
   count_launch();
   const size_t blocks = (n + 1023) / 1024;
   radam_dev_kernel<<<(unsigned)(blocks > 1184 ? 1184 : blocks), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, hyper);
-  count_launch();
-  ZCHECK_LAUNCH();
-  return ZEGGS_OK;
-}
-
-extern "C" int zeggs_radam_step(float* p, const float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2,
-                                float eps, int step, float grad_scale, void* stream) {
-  ZCHECK_ARG(p && g && m && v && step >= 1, "radam: bad arguments");
-  if (n == 0) return ZEGGS_OK;
-  const double b2t = pow((double)beta2, (double)step);
-  const double n_max = 2.0 / (1.0 - (double)beta2) - 1.0;
-  const double n_sma = n_max - 2.0 * step * b2t / (1.0 - b2t);            // :66-68
-  double step_size; int adaptive;
-  if (n_sma >= 5.0) {
-    step_size = sqrt((1.0 - b2t) * (n_sma - 4.0) / (n_max - 4.0) * (n_sma - 2.0) / n_sma * n_max / (n_max - 2.0)) /
-                (1.0 - pow((double)beta1, (double)step));                 // :72-76
-    adaptive = 1;
-  } else {
-    step_size = 1.0 / (1.0 - pow((double)beta1, (double)step));           // :77-78
-    adaptive = 0;
-  }
-  ScopedTimer tm("optimizer", (cudaStream_t)stream);
-  const size_t blocks = (n + 1023) / 1024;
-  radam_kernel<<<(unsigned)(blocks > 1184 ? 1184 : blocks), 256, 0, (cudaStream_t)stream>>>(
-      p, g, m, v, n, beta1, beta2, eps, (float)(step_size * (double)lr), adaptive, grad_scale);
   count_launch();
   ZCHECK_LAUNCH();
   return ZEGGS_OK;

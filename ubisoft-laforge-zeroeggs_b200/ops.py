@@ -205,6 +205,7 @@ def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
     after the weight packs (decoder_prepack)."""
     H, S, Z = dec.hidden_size, dec.speech_encoding_size, dec.style_encoding_size
     film = dec.film
+    kind = "_film" if film else ""
     l = _lib.lib()
     w = [_f32c(p, dev) for p in dec._weights()]
     names = ["W0", "b0", "W_ih0", "b_ih0", "W_hh0", "b_hh0", "W_ih1", "b_ih1", "W_hh1", "b_hh1", "W2", "b2",
@@ -220,22 +221,14 @@ def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
     for n, t in tensors.items():
         setattr(a, n, _lib.ptr(t))
         keep.append(t)
+    use_tc = resolve_engine(H, S, Z, film)          # a FiLM decoder: fp32, or raises on an explicit "tc"
+    args = a
     if film:
-        resolve_engine(H, S, Z, film=True)           # raises on an explicit "tc"
-        f = _lib.DecoderFilmFwdArgs(dec=a)
+        args = _lib.DecoderFilmFwdArgs(dec=a)
         for n, t in zip(_FILM_NAMES, w[18:]):
-            setattr(f, n, _lib.ptr(t))
-        f.dec.packed = _weight_pack(dec, "_film", f, dev).data_ptr()
-        keep.append(dec.__dict__["_zeggs_packed_film"][1])
-        if pack_only:
-            return f, keep, None
-        wsb = l.zeggs_decoder_film_workspace_bytes(B, T, H, S, Z, int(save))
-        ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if save else WS.get("dec_fwd", wsb, dev)
-        f.dec.workspace, f.dec.workspace_bytes, f.dec.save_for_backward = ws.data_ptr(), wsb, int(save)
-        keep.append(ws)
-        return f, keep, ws
+            setattr(args, n, _lib.ptr(t))
+        a = args.dec                                 # a view of the copy inside args
     # each engine packs only its own slices
-    use_tc = resolve_engine(H, S, Z)
     if use_tc and B > 32:
         raise _lib.ZeggsError("tensor-core decoder engine: one call covers one 32-sample batch tile (decoder_window splits larger batches)")
     if use_tc:
@@ -244,18 +237,18 @@ def _decoder_args(dec, B, T, dev, tensors, stats, dt, save, pack_only=False):
         a.engine, a.packed_tc, a.workspace_tc = 1, ptc.data_ptr(), wtc.data_ptr()
         keep += [ptc, wtc]
     else:
-        packed = _weight_pack(dec, "", a, dev)
+        packed = _weight_pack(dec, kind, args, dev)
         a.packed = packed.data_ptr()
         keep.append(packed)
     if pack_only:
-        return a, keep, None
-    wsb = l.zeggs_decoder_workspace_bytes(B, T, H, S, Z, int(save))
+        return args, keep, None
+    wsb = getattr(l, f"zeggs_decoder{kind}_workspace_bytes")(B, T, H, S, Z, int(save))
     ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if save else WS.get("dec_fwd", wsb, dev)
     a.workspace = ws.data_ptr()
     a.workspace_bytes = wsb
     a.save_for_backward = int(save)
     keep.append(ws)
-    return a, keep, ws
+    return args, keep, ws
 
 
 def decoder_prepack(dec, B, T, dev, stats, dt, backward=True):
@@ -314,11 +307,12 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
     encoders' backward passes on other streams / lanes in between."""
     l = _lib.lib()
     fa, keep, ws = state
-    a = fa.dec if dec.film else fa
+    film = dec.film
+    kind = "_film" if film else ""
+    fb = _lib.DecoderFilmBwdArgs() if film else _lib.DecoderBwdArgs()
+    a, b = (fa.dec, fb.dec) if film else (fa, fb)
     dev = ws.device
     B, T, H, S, Z = a.B, a.T, a.H, a.S, a.Z
-    fb = _lib.DecoderFilmBwdArgs() if dec.film else None
-    b = fb.dec if dec.film else _lib.DecoderBwdArgs()
     hold = []
     for name, g in (("dY", dY), ("dRootPos", dRp), ("dRootRot", dRq)):
         if g is not None:
@@ -326,17 +320,13 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
             hold.append(g)
             setattr(b, name, g.data_ptr())
     # transposed weight slices for the backward recurrence
-    if dec.film:
-        packed = _weight_pack(dec, "_bwd_film", fa, dev)
-        b.packed_bwd = packed.data_ptr()
-        hold.append(packed)
-    elif a.engine == 1:
+    if a.engine == 1:
         ptc = _weight_pack(dec, "_bwd_tc", a, dev)
         wtc = WS.get("dec_bwd_tc", l.zeggs_decoder_bwd_tc_workspace_bytes(H, S, Z), dev)
         b.packed_bwd_tc, b.workspace_tc = ptc.data_ptr(), wtc.data_ptr()
         hold += [ptc, wtc]
     else:
-        packed = _weight_pack(dec, "_bwd", a, dev)
+        packed = _weight_pack(dec, "_bwd" + kind, fa, dev)
         b.packed_bwd = packed.data_ptr()
         hold.append(packed)
     grads = _grad_targets(dec._weights(), grads_out)
@@ -347,11 +337,11 @@ def decoder_window_backward(dec, state, dY, dRp, dRq, grads_out=None, split=Fals
     dSpeech = torch.empty((B, T, S), dtype=torch.float32, device=dev)
     dStyle = torch.empty((B, T, Z), dtype=torch.float32, device=dev)
     b.dSpeech, b.dStyle = dSpeech.data_ptr(), dStyle.data_ptr()
-    wsb = (l.zeggs_decoder_film_bwd_workspace_bytes if dec.film else l.zeggs_decoder_bwd_workspace_bytes)(B, T, H, S, Z)
+    wsb = getattr(l, f"zeggs_decoder{kind}_bwd_workspace_bytes")(B, T, H, S, Z)
     bws = WS.get("dec_bwd", wsb, dev)
     b.workspace, b.workspace_bytes = bws.data_ptr(), wsb
-    name = "zeggs_decoder_film_window_bwd" if dec.film else "zeggs_decoder_window_bwd"
-    run = (lambda: getattr(l, name)(fa, fb, _lib.stream_ptr())) if dec.film else (lambda: getattr(l, name)(a, b, _lib.stream_ptr()))
+    name = f"zeggs_decoder{kind}_window_bwd"
+    run = lambda: getattr(l, name)(fa, fb, _lib.stream_ptr())
     if not split:
         _lib.check(run(), name)
         return grads, dSpeech, dStyle
@@ -742,31 +732,6 @@ def pose_to_bvh_channels(root_pos, root_rot, lpos, ltxy, start_position=(0.0, 0.
         a.start_rot[i] = float(start_rotation[i])
     _lib.check(_lib.lib().zeggs_pose_to_bvh_channels(a, _lib.stream_ptr()), "zeggs_pose_to_bvh_channels")
     return (pos, eul, lrot) if want_lrot else (pos, eul)
-
-
-# ---------------------------------------------------------------------------------------------- single decoder step
-def decoder_step(dec, pose, speech, style, state):
-    """RecurrentDecoderNormal.forward (modules.py:179-185) for one frame, fp32: pose [B,1134] normalised input vector, speech [B,S],
-    style [B,Z], state [2,B,H] -> (y [B,1131] normalised, new state [2,B,H])."""
-    if pose.device.type != "cuda":
-        raise _lib.ZeggsError("decoder_step runs on CUDA tensors only (no CPU fallback)")
-    if dec.film:
-        raise _lib.ZeggsError("decoder_step covers the normal decoder (RecurrentDecoderNormal); run a FiLM decoder through decoder_window")
-    l = _lib.lib()
-    dev = pose.device
-    w = [_f32c(p, dev) for p in dec._weights()[:12]]
-    pose, speech, style, state = _f32c(pose), _f32c(speech), _f32c(style), _f32c(state)
-    B, H, S, Z = pose.shape[0], dec.hidden_size, speech.shape[1], style.shape[1]
-    y = torch.empty((B, P_OUT), dtype=torch.float32, device=dev)
-    h_out = torch.empty((2, B, H), dtype=torch.float32, device=dev)
-    wsb = l.zeggs_decoder_step_workspace_bytes(B, H, S, Z)
-    ws = WS.get("dec_step", wsb, dev)
-    a = _lib.DecoderStepArgs(B=B, H=H, S=S, Z=Z, pose=pose.data_ptr(), speech=speech.data_ptr(), style=style.data_ptr(),
-                             h_in=state.data_ptr(), y=y.data_ptr(), h_out=h_out.data_ptr(), workspace=ws.data_ptr(), workspace_bytes=wsb)
-    for n, t in zip(("W0", "b0", "W_ih0", "b_ih0", "W_hh0", "b_hh0", "W_ih1", "b_ih1", "W_hh1", "b_hh1", "W2", "b2"), w):
-        setattr(a, n, t.data_ptr())
-    _lib.check(l.zeggs_decoder_step_fwd(a, _lib.stream_ptr()), "zeggs_decoder_step_fwd")
-    return y, h_out
 
 
 # ---------------------------------------------------------------------------------------------- training-set construction

@@ -1,7 +1,7 @@
 """RAdam with the reference's constructor surface (ZEGGS/optimizers.py) backed by one fused kernel.
 
 All parameters are re-homed into ONE flat fp32 buffer (each nn.Parameter becomes a view of it), with a
-matching flat gradient buffer: the optimizer step is a single launch of zeggs_radam_step and the
+matching flat gradient buffer: the optimizer step is one zeggs_radam_step_dev call (two launches) and the
 data-parallel gradient exchange is a single NCCL all-reduce of `flat_grad`."""
 import torch
 
