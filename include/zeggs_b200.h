@@ -292,7 +292,8 @@ int zeggs_style_enc_bwd(const zeggs_style_enc_args* a, const zeggs_style_enc_gra
  * Only output[:, -1] is consumed, so the forward direction runs all T steps (one persistent cooperative kernel) while the
  * reverse direction is the single GRU cell at t = T-1 from h = 0: W_hh_r is not read and dW_hh_r is written as zeros (the
  * reference's autograd gives it exactly zero).  E = 2 * style_embedding_size with the VAE, style_embedding_size without.
- * Supported hidden sizes: H % 4 == 0 and H <= 528, or H % 8 == 0 and H <= 1056.  _bwd needs the forward's workspace untouched.
+ * Supported hidden sizes: H % 4 == 0 and H <= 528, H % 8 == 0 and H <= 1056, or H % 16 == 0 and H <= 2112 (16 units per CTA,
+ * W_hh read from global memory every step; one call takes at most 1792 samples there).  _bwd needs the forward's workspace untouched.
  */
 typedef struct {
   int B, T, C_in, H, E;

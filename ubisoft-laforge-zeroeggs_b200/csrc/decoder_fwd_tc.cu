@@ -606,7 +606,9 @@ __global__ void __launch_bounds__(256) fold_finish_kernel(zeggs_decoder_fwd_args
     float p = 0.f;
     if (n < P_OUT) {
       p = w.YC[((size_t)(t - 1) * 32 + b) * P_OUT + n] * os + om;
-      if (n < 6) p = w.Y6[((size_t)t * 32 + b) * 8 + n];
+      // Y6 holds live samples only: a padding lane b >= B takes 0, not the stale workspace (its x_pose column multiplies zero
+      // gradients in dW0 / dW_ih0, where a stale NaN would still poison the product)
+      if (n < 6) p = b < a.B ? w.Y6[((size_t)t * 32 + b) * 8 + n] : 0.f;
       if (b < a.B) a.Y[((size_t)b * T + t) * P_OUT + n] = p;
     }
     tile[b][tx] = p;

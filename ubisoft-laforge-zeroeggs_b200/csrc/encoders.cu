@@ -104,10 +104,11 @@ __global__ void layernorm_bwd_kernel(const float* __restrict__ dy, const float* 
 }
 // Column reductions over many rows in ONE launch (deterministic): grid (ceil(D/32), RB), block (32,8); every block writes its
 // partial[rb][2][D] sums, the LAST block to arrive for a column group (device counter, reset by that block so the next launch finds
-// zeros) adds the RB partials in a fixed order.  mode 0: out0 = sum_r a[r][d];  mode 1: out0 = sum a*b, out1 = sum a.
+// zeros) adds the RB partials in a fixed order.  mode 0: out0 = sum_r a[r][d];  mode 1: out0 = sum a*b, out1 = sum a.  Rows of a and b
+// are ld apart (ld >= D: a slab of a wider matrix).
 constexpr int COLRED_RB = 64;
 constexpr int COLRED_MAXD = 4096;
-__global__ void colred_kernel(const float* __restrict__ a, const float* __restrict__ b, int rows, int D, float* partial, int* counters,
+__global__ void colred_kernel(const float* __restrict__ a, const float* __restrict__ b, int rows, int D, int ld, float* partial, int* counters,
                               float* __restrict__ out0, float* __restrict__ out1) {
   __shared__ float s0[8][33], s1[8][33];
   __shared__ int last;
@@ -122,13 +123,13 @@ __global__ void colred_kernel(const float* __restrict__ a, const float* __restri
     for (; r + 24 < r_hi; r += 32) {
       float v[4], w[4];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) { v[u] = a[(size_t)(r + 8 * u) * D + d]; w[u] = b ? b[(size_t)(r + 8 * u) * D + d] : 1.f; }
+      for (int u = 0; u < 4; ++u) { v[u] = a[(size_t)(r + 8 * u) * ld + d]; w[u] = b ? b[(size_t)(r + 8 * u) * ld + d] : 1.f; }
 #pragma unroll
       for (int u = 0; u < 4; ++u) { xa[u] += v[u] * w[u]; ya[u] += v[u]; }
     }
     for (; r < r_hi; r += 8) {
-      const float v = a[(size_t)r * D + d];
-      xa[0] += b ? v * b[(size_t)r * D + d] : v; ya[0] += v;
+      const float v = a[(size_t)r * ld + d];
+      xa[0] += b ? v * b[(size_t)r * ld + d] : v; ya[0] += v;
     }
     x = (xa[0] + xa[1]) + (xa[2] + xa[3]); y = (ya[0] + ya[1]) + (ya[2] + ya[3]);
   }
@@ -250,12 +251,20 @@ static int ew_add(float* dst, const float* a, const float* b, size_t n, size_t p
   ew_add_kernel<<<GRID1(n), 256, 0, s>>>(dst, a, b, n, period); LAUNCH_OK(); return 0; }
 static int ln_fwd(const float* a, const float* res, const float* g, const float* b, int rows, int D, float* y, float* xh, float* rs, cudaStream_t s) {
   layernorm_fwd_kernel<<<ceil_div(rows, 8), 256, 0, s>>>(a, res, g, b, rows, D, y, xh, rs); LAUNCH_OK(); return 0; }
-// red: the column reductions' scratch inside the calling module's workspace, [COLRED_RB][2][D <= 4096] partials + arrival counters
+// red: the column reductions' scratch inside the calling module's workspace, [COLRED_RB][2][4096] partials + arrival counters.
+// Wider sums (the GRU's 3H bias columns above H = 1365) run as consecutive slabs of at most 4096 columns through the same scratch:
+// stream order keeps a slab's partials until its last block has read them, and that block leaves the counters at zero.
 static int colred(const float* a, const float* b, int rows, int D, float* out0, float* out1, float* red, cudaStream_t s) {
-  ZCHECK_ARG(red != nullptr && D <= COLRED_MAXD, "column reduction: scratch missing or D=%d too wide", D);
+  ZCHECK_ARG(red != nullptr, "column reduction: scratch missing");
   const int RB = rows < 8 * COLRED_RB ? ceil_div(rows, 8) : COLRED_RB;
   int* counters = reinterpret_cast<int*>(red + (size_t)COLRED_RB * 2 * COLRED_MAXD);
-  colred_kernel<<<dim3(ceil_div(D, 32), RB), dim3(32, 8), 0, s>>>(a, b, rows, D, red, counters, out0, out1); LAUNCH_OK(); return 0; }
+  for (int d0 = 0; d0 < D; d0 += COLRED_MAXD) {
+    const int w = std::min(COLRED_MAXD, D - d0);
+    colred_kernel<<<dim3(ceil_div(w, 32), RB), dim3(32, 8), 0, s>>>(a + d0, b ? b + d0 : nullptr, rows, w, D, red, counters, out0 + d0,
+                                                                     out1 ? out1 + d0 : nullptr);
+    LAUNCH_OK();
+  }
+  return 0; }
 // the arrival counters behind the partials must be zero before the first reduction of a call (the workspace is caller memory)
 static int colred_reset(float* red, cudaStream_t s) {
   ZCHECK_CUDA(cudaMemsetAsync(red + (size_t)COLRED_RB * 2 * COLRED_MAXD, 0, (COLRED_MAXD / 32) * sizeof(int), s)); return 0; }
@@ -519,7 +528,8 @@ extern "C" int zeggs_style_enc_gru_fwd(const zeggs_style_enc_gru_args* ap, void*
   const bool vae = a.mu != nullptr;
   ZCHECK_ARG(B >= 1 && T >= 1 && Cin >= 1 && E >= 1 && (!vae || E % 2 == 0) && a.x && a.z && (a.logvar != nullptr) == vae,
              "style_enc_gru: bad arguments");
-  ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru: hidden size %d unsupported (H %% 4 == 0 and H <= 528, or H %% 8 == 0 and H <= 1056)", H);
+  ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru: hidden size %d unsupported (H %% 4 == 0 and H <= 528, H %% 8 == 0 and H <= 1056, "
+             "or H %% 16 == 0 and H <= 2112)", H);
   ZCHECK_ARG(B <= style_gru_max_batch(H), "style_enc_gru: batch %d too large: at hidden size %d the backward's shared memory holds at "
              "most %d samples per call", B, H, style_gru_max_batch(H));
   StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);

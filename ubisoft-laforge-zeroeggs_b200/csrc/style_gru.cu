@@ -15,6 +15,9 @@
 //            gradients dG_ih(t), dG_hh(t) of its units; grid barrier; phase B reads the whole dG_hh(t) and forms
 //            dh(t-1) = dh(t) * z + dG_hh(t) W_hh for its own units -- which is exactly what phase A of step t-1 needs: one barrier per
 //            step again.
+//   U = 16 (1056 < H <= 2112): W_hh is 3H^2 fp32 (53.5 MB at H = 2112) against ~30 MB of shared memory on all SMs together, so
+//            neither kernel keeps it resident: each K chunk's slice of the CTA's rows (forward) or columns (BPTT) is read from global
+//            memory (through L2) into shared memory next to the staged operand chunk, every step.  Same products, same order.
 // The K dimension of each per-step product is staged through shared memory in 512-row chunks ([k][33] fp32, conflict-free for
 // 32 batch lanes; every thread has 8 global loads in flight per round, since the step is bound by the latency of this exchange);
 // batches larger than 32 loop over 32-sample tiles.
@@ -44,16 +47,69 @@ __device__ __forceinline__ void gru_stage(float* __restrict__ dst, const float* 
   }
 }
 
-// units per CTA: 4 while the grid fits one CTA per SM of the H100 (H <= 528), else 8 (H <= 1056); 0 = unsupported
+// U = 16: row stride of the forward's streamed W_hh chunk [KC][GRU_WS], 3U = 48 padded to 52 so that a warp's staging stores
+// (16 rows x 2 float4 columns) land in 32 distinct banks, and rows stay 16-byte aligned for the float4 reads of the product
+constexpr int GRU_WS = 52;
+
+// W_hh may sit at any 4-byte offset (TrainStep packs all parameters into one flat buffer), so global reads are scalar; a thread reads
+// 4 consecutive floats of a row per item and keeps 8 items (32 loads) in flight.
+__device__ __forceinline__ float4 ldg4_any(const float* p) { return make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3)); }
+
+// Ws[kk][g*16 + u] (row stride GRU_WS) = W_hh[g*H + j0 + u][k0 + kk] for the 48 rows of the CTA's 16 units, kk < kc (kc % 16 == 0).
+// Lane bits: 1 for the 4 floats along k, 4 for the row, so a warp reads 16 rows x 32 bytes.
+__device__ __forceinline__ void gru_stage_rows16(float* __restrict__ dst, const float* __restrict__ W, int H, int j0, int k0, int kc) {
+  const int n = 12 * kc;                   // items of 4 floats: 48 rows x kc/4
+  for (int i0 = threadIdx.x; i0 < n; i0 += GRU_THREADS * 8) {
+    float4 v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int i = i0 + e * GRU_THREADS, rest = i >> 5, g = rest % 3, u = (i >> 1) & 15, k = 4 * (2 * (rest / 3) + (i & 1));
+      v[e] = i < n ? ldg4_any(W + (size_t)(g * H + j0 + u) * H + k0 + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int i = i0 + e * GRU_THREADS, rest = i >> 5, g = rest % 3, u = (i >> 1) & 15, k = 4 * (2 * (rest / 3) + (i & 1));
+      if (i < n) {
+        float* d = dst + k * GRU_WS + g * 16 + u;
+        d[0] = v[e].x; d[GRU_WS] = v[e].y; d[2 * GRU_WS] = v[e].z; d[3 * GRU_WS] = v[e].w;
+      }
+    }
+  }
+}
+
+// Wc[kk][u] = W_hh[r0 + kk][j0 + u] for the CTA's 16 columns, kk < kc: 64 contiguous bytes per row, stored as they are read
+__device__ __forceinline__ void gru_stage_cols16(float* __restrict__ dst, const float* __restrict__ W, int H, int j0, int r0, int kc) {
+  const int n = 4 * kc;
+  for (int i0 = threadIdx.x; i0 < n; i0 += GRU_THREADS * 8) {
+    float4 v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int i = i0 + e * GRU_THREADS;
+      v[e] = i < n ? ldg4_any(W + (size_t)(r0 + (i >> 2)) * H + j0 + 4 * (i & 3)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int i = i0 + e * GRU_THREADS;
+      if (i < n) reinterpret_cast<float4*>(dst)[i] = v[e];
+    }
+  }
+}
+
+// units per CTA: 4 while the grid fits one CTA per SM of the H100 (H <= 528), else 8 (H <= 1056), else 16 (H <= 2112); 0 = unsupported
 int style_gru_units(int H) {
   if (H % 4 == 0 && H / 4 <= 132) return 4;
   if (H % 8 == 0 && H / 8 <= 132) return 8;
+  if (H % 16 == 0 && H / 16 <= 132) return 16;
   return 0;
 }
 
-// dynamic shared memory per CTA: the forward kernel's with nbt = 0, the BPTT kernel's with its nbt 32-sample tiles of carry
+// dynamic shared memory per CTA: the forward kernel's with nbt = 0, the BPTT kernel's with its nbt 32-sample tiles of carry.
+// U = 16 keeps no weights resident: the forward holds one [KC][GRU_WS] chunk of W_hh rows, the BPTT one [KC][U] chunk of columns.
 template <int U>
 static size_t gru_smem_bytes(int H, int nbt) {
+  if (U == 16)
+    return (size_t)(nbt == 0 ? GRU_KC * GRU_WS + GRU_KC * 33 + 8 * 3 * U * 32
+                             : GRU_KC * U + GRU_KC * 33 + 8 * U * 32 + nbt * U * 32) * sizeof(float);
   return (size_t)(3 * U * H + GRU_KC * 33 + 8 * 3 * U * 32 + nbt * U * 32) * sizeof(float);
 }
 
@@ -65,8 +121,9 @@ constexpr size_t GRU_SMEM_LIMIT = 232448;
 int style_gru_max_batch(int H) {
   const int U = style_gru_units(H);
   if (U == 0) return 0;
+  auto bytes = [&](int nbt) { return U == 4 ? gru_smem_bytes<4>(H, nbt) : U == 8 ? gru_smem_bytes<8>(H, nbt) : gru_smem_bytes<16>(H, nbt); };
   int nbt = 0;
-  while ((U == 4 ? gru_smem_bytes<4>(H, nbt + 1) : gru_smem_bytes<8>(H, nbt + 1)) <= GRU_SMEM_LIMIT) ++nbt;
+  while (bytes(nbt + 1) <= GRU_SMEM_LIMIT) ++nbt;
   return 32 * nbt;
 }
 
@@ -79,15 +136,18 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_fwd_kernel(int B, int T, i
                                                                  float* Hs, float* __restrict__ Gs, float* __restrict__ hcat,
                                                                  unsigned* bar) {
   constexpr int R = 3 * U;
+  constexpr bool STREAM = U == 16;        // W_hh read per K chunk (see the top of the file)
+  constexpr int WS = STREAM ? GRU_WS : R;
   extern __shared__ __align__(16) float sm[];
-  float* Ws = sm;                         // [H][R]: Ws[k*R + g*U + u] = W_hh[g*H + c*U + u][k]
-  float* hs = Ws + (size_t)R * H;         // [KC][33]
+  float* Ws = sm;                         // [H][R]: Ws[k*R + g*U + u] = W_hh[g*H + c*U + u][k]; streamed: rows k0 .. k0+kc-1, stride WS
+  float* hs = Ws + (STREAM ? (size_t)GRU_KC * WS : (size_t)R * H);   // [KC][33]
   float* red = hs + GRU_KC * 33;          // [8][R][32]
   const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < R * H; i += GRU_THREADS) {
-    const int r = i / H, k = i - r * H, g = r / U, u = r - g * U;
-    Ws[(size_t)k * R + r] = Whh[(size_t)(g * H + c * U + u) * H + k];
-  }
+  if constexpr (!STREAM)
+    for (int i = tid; i < R * H; i += GRU_THREADS) {
+      const int r = i / H, k = i - r * H, g = r / U, u = r - g * U;
+      Ws[(size_t)k * R + r] = Whh[(size_t)(g * H + c * U + u) * H + k];
+    }
   GridBarrier gb; gb.counter = bar; gb.error = bar + 1; gb.epoch = 0; gb.nblocks = gridDim.x;
   const int H3 = 3 * H;
   for (int t = 0; t < T; ++t) {
@@ -100,11 +160,12 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_fwd_kernel(int B, int T, i
         const int kc = min(GRU_KC, H - k0);
         __syncthreads();
         gru_stage(hs, hprev, H, B, b0, k0, kc);
+        if constexpr (STREAM) gru_stage_rows16(Ws, Whh, H, c * U, k0, kc);
         __syncthreads();
         const int kw = (kc + 7) / 8, kend = min(kc, warp * kw + kw);
         for (int kk = warp * kw; kk < kend; ++kk) {
           const float hv = hs[kk * 33 + lane];
-          const float4* w4 = reinterpret_cast<const float4*>(Ws + (size_t)(k0 + kk) * R);
+          const float4* w4 = reinterpret_cast<const float4*>(Ws + (size_t)((STREAM ? 0 : k0) + kk) * WS);
 #pragma unroll
           for (int q = 0; q < R / 4; ++q) {
             const float4 w = w4[q];
@@ -153,16 +214,18 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_bwd_kernel(int B, int T, i
                                                                  const float* __restrict__ dhf, int ld_dhf, float* __restrict__ dGih,
                                                                  float* dGhh, unsigned* bar) {
   extern __shared__ __align__(16) float sm[];
+  constexpr bool STREAM = U == 16;         // W_hh read per K chunk (see the top of the file)
   const int H3 = 3 * H, nbt = (B + 31) / 32;
-  float* Wc = sm;                          // [3H][U]: Wc[row*U + u] = W_hh[row][c*U + u]
-  float* ds = Wc + (size_t)H3 * U;         // [KC][33]
-  float* red = ds + GRU_KC * 33;           // [8][U][32]  (room for 3U reserved by gru_smem_bytes)
-  float* carry = red + 8 * 3 * U * 32;     // [nbt][U][32]: dh of the own units
+  float* Wc = sm;                          // [3H][U]: Wc[row*U + u] = W_hh[row][c*U + u]; streamed: rows r0 .. r0+kc-1
+  float* ds = Wc + (size_t)(STREAM ? GRU_KC : H3) * U;       // [KC][33]
+  float* red = ds + GRU_KC * 33;           // [8][U][32]  (room for 3U reserved by gru_smem_bytes below U = 16)
+  float* carry = red + 8 * (STREAM ? 1 : 3) * U * 32;        // [nbt][U][32]: dh of the own units
   const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < H3 * U; i += GRU_THREADS) {
-    const int row = i / U, u = i - row * U;
-    Wc[i] = Whh[(size_t)row * H + c * U + u];
-  }
+  if constexpr (!STREAM)
+    for (int i = tid; i < H3 * U; i += GRU_THREADS) {
+      const int row = i / U, u = i - row * U;
+      Wc[i] = Whh[(size_t)row * H + c * U + u];
+    }
   for (int i = tid; i < nbt * U * 32; i += GRU_THREADS) {
     const int bt = i / (U * 32), u = (i >> 5) % U, bl = i & 31, b = bt * 32 + bl;
     carry[i] = b < B ? dhf[(size_t)b * ld_dhf + c * U + u] : 0.f;
@@ -200,11 +263,12 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_bwd_kernel(int B, int T, i
         const int kc = min(GRU_KC, H3 - r0);
         __syncthreads();
         gru_stage(ds, dg, H3, B, b0, r0, kc);
+        if constexpr (STREAM) gru_stage_cols16(Wc, Whh, H, c * U, r0, kc);
         __syncthreads();
         const int kw = (kc + 7) / 8, kend = min(kc, warp * kw + kw);
         for (int kk = warp * kw; kk < kend; ++kk) {
           const float dv = ds[kk * 33 + lane];
-          const float4* w4 = reinterpret_cast<const float4*>(Wc + (size_t)(r0 + kk) * U);
+          const float4* w4 = reinterpret_cast<const float4*>(Wc + (size_t)((STREAM ? 0 : r0) + kk) * U);
 #pragma unroll
           for (int q = 0; q < U / 4; ++q) {
             const float4 w = w4[q];
@@ -264,11 +328,13 @@ __global__ void rev_cell_bwd_kernel(int B, int H, const float* __restrict__ GIr,
 int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
                          unsigned* bar, cudaStream_t s) {
   const int U = style_gru_units(H);
-  ZCHECK_ARG(U > 0 && B >= 1 && T >= 1, "style GRU: hidden size %d unsupported (need H %% 4 == 0, H <= 528, or H %% 8 == 0, H <= 1056)", H);
+  ZCHECK_ARG(U > 0 && B >= 1 && T >= 1, "style GRU: hidden size %d unsupported (need H %% 4 == 0, H <= 528, H %% 8 == 0, H <= 1056, "
+             "or H %% 16 == 0, H <= 2112)", H);
   ZCHECK_CUDA(cudaMemsetAsync(bar, 0, 2 * sizeof(unsigned), s));
   ZCHECK_CUDA(cudaMemsetAsync(Hs, 0, (size_t)B * H * sizeof(float), s));     // h(-1) = 0
   if (U == 4) return launch_persistent(gru_fwd_kernel<4>, H / 4, GRU_THREADS, gru_smem_bytes<4>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
-  return launch_persistent(gru_fwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
+  if (U == 8) return launch_persistent(gru_fwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
+  return launch_persistent(gru_fwd_kernel<16>, H / 16, GRU_THREADS, gru_smem_bytes<16>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
 }
 
 int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs, const float* Gs, const float* dhf, int ld_dhf,
@@ -281,7 +347,9 @@ int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs,
   const int nbt = (B + 31) / 32;
   if (U == 4)
     return launch_persistent(gru_bwd_kernel<4>, H / 4, GRU_THREADS, gru_smem_bytes<4>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
-  return launch_persistent(gru_bwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
+  if (U == 8)
+    return launch_persistent(gru_bwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
+  return launch_persistent(gru_bwd_kernel<16>, H / 16, GRU_THREADS, gru_smem_bytes<16>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
 }
 
 int style_gru_rev_cell_fwd(int B, int H, const float* GIr, const float* bhh, float* hcat, cudaStream_t s) {
