@@ -42,10 +42,12 @@ __global__ void __launch_bounds__(MEL_WARPS * 32, 2) mel_kernel(zeggs_mel_args a
   const short* wav16 = a.wav_i16 ? a.wav_i16 + (size_t)clip * a.n_samples : nullptr;
   const float gain = a.gain ? __ldg(a.gain + clip) : 1.0f;        // loudness normalisation folded into the load
   const int Ts = a.n_samples, Te = Ts < n_fft ? n_fft : Ts;     // spectrograms.py:233-234 zero-extends short clips
+  // the 16-byte paths also need a 16-byte aligned base: a contiguous view with a storage offset need not have one
+  const bool base16 = ((reinterpret_cast<uintptr_t>(a.wav ? (const void*)a.wav : (const void*)a.wav_i16) & 15) == 0);
   // ---- stage the tile's samples (reflect padding, spectrograms.py:237-239)
   {
     const int o0 = f0 * hop - n_fft / 2;
-    if (wav && o0 >= 0 && o0 + nsamp_tile <= Ts && ((o0 & 3) == 0) && ((a.n_samples & 3) == 0) && ((nsamp_tile & 3) == 0)) {
+    if (wav && base16 && o0 >= 0 && o0 + nsamp_tile <= Ts && ((o0 & 3) == 0) && ((a.n_samples & 3) == 0) && ((nsamp_tile & 3) == 0)) {
       // interior tile: straight 16-byte copies
       const float4* src4 = reinterpret_cast<const float4*>(wav + o0);
       float4* dst4 = reinterpret_cast<float4*>(samp);
@@ -54,7 +56,7 @@ __global__ void __launch_bounds__(MEL_WARPS * 32, 2) mel_kernel(zeggs_mel_args a
         v.x *= gain; v.y *= gain; v.z *= gain; v.w *= gain;
         dst4[i] = v;
       }
-    } else if (wav16 && o0 >= 0 && o0 + nsamp_tile <= Ts && ((o0 & 7) == 0) && ((a.n_samples & 7) == 0) && ((nsamp_tile & 7) == 0)) {
+    } else if (wav16 && base16 && o0 >= 0 && o0 + nsamp_tile <= Ts && ((o0 & 7) == 0) && ((a.n_samples & 7) == 0) && ((nsamp_tile & 7) == 0)) {
       // interior tile of int16 PCM: 16-byte loads of 8 samples, x / 32768 (audio_files.py:211-236)
       const uint4* src8 = reinterpret_cast<const uint4*>(wav16 + o0);
       const float sc = gain * (1.0f / 32768.0f);
@@ -228,6 +230,7 @@ extern "C" int zeggs_mel_forward(const zeggs_mel_args* ap, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (a.n_fft != 2 * MEL_N2) { set_error("mel: n_fft=%d unsupported (this build transforms n_fft=800 only)", a.n_fft); return ZEGGS_ERR_UNSUPPORTED; }
   ZCHECK_ARG(a.n_clips >= 0 && a.n_samples >= 1 && a.hop >= 1 && a.hop <= 800 && a.n_mels >= 1 && a.n_mels <= 256, "mel: bad shape");
+  ZCHECK_ARG(a.n_clips <= 65535, "mel: n_clips=%d exceeds 65535, the grid's y limit (one grid row per clip); split the batch", a.n_clips);
   ZCHECK_ARG((a.wav != nullptr) != (a.wav_i16 != nullptr), "mel: exactly one of wav (f32) / wav_i16 (int16 PCM)");
   ZCHECK_ARG(a.window && a.twiddle && a.fb_start && a.fb_len && a.fb_off && a.fb_w, "mel: null table/input pointer");
   ZCHECK_ARG(a.mel_out || a.feat_out, "mel: no output requested");
@@ -241,13 +244,22 @@ extern "C" int zeggs_mel_forward(const zeggs_mel_args* ap, void* stream_) {
                "mel: anim_length %d needs frames beyond L=%d (reference would produce NaN, data_pipeline.py:473)", a.anim_length, L);
   }
   const int nsamp_tile = (MEL_FT + 1) * a.hop + a.n_fft;
-  size_t smem = (size_t)(((nsamp_tile + 3) & ~3) + (MEL_FT + 2) * a.n_mels * (a.mel_out ? 2 : 1) + ((MEL_FT + 2 + 3) & ~3)) * sizeof(float)
-              + (size_t)24 * 32 * sizeof(float2) + (size_t)MEL_WARPS * MEL_TB * sizeof(C2)
-              + (size_t)((((a.fb_total > 0 && a.fb_total <= 4096 ? a.fb_total : 0) + 3) & ~3) + 3 * a.n_mels) * sizeof(float);
+  const size_t smem_rest = (size_t)(((nsamp_tile + 3) & ~3) + (MEL_FT + 2) * a.n_mels * (a.mel_out ? 2 : 1) + ((MEL_FT + 2 + 3) & ~3)) * sizeof(float)
+                         + (size_t)24 * 32 * sizeof(float2) + (size_t)MEL_WARPS * MEL_TB * sizeof(C2) + (size_t)3 * a.n_mels * sizeof(int);
+  const size_t smem_fb = (size_t)(((a.fb_total > 0 && a.fb_total <= 4096 ? a.fb_total : 0) + 3) & ~3) * sizeof(float);
+  DeviceLimits lim;
+  RC(device_limits(&lim));
+  // Large hops with many bands and mel_out (hop 800, 256 bands: 233,088 B with the shipped 752 weights) exceed the
+  // opt-in limit (232,448 B on an H100): there the kernel reads the filterbank weights from global memory instead.
+  zeggs_mel_args la = a;
+  size_t smem = smem_rest + smem_fb;
+  if (smem > lim.smem_optin) { la.fb_total = 0; smem = smem_rest; }
+  ZCHECK_ARG(smem <= lim.smem_optin, "mel: hop=%d with n_mels=%d needs %zu B of shared memory per block, above the device's %zu B",
+             a.hop, a.n_mels, smem, lim.smem_optin);
   RC(set_max_dynamic_smem(mel_kernel, smem));
   dim3 grid(ceil_div(L, MEL_FT), a.n_clips);
   ScopedTimer tm("mel", stream);
-  mel_kernel<<<grid, MEL_WARPS * 32, smem, stream>>>(a, L, a.frames_per_anim);
+  mel_kernel<<<grid, MEL_WARPS * 32, smem, stream>>>(la, L, a.frames_per_anim);
   count_launch();
   ZCHECK_LAUNCH();
   return ZEGGS_OK;
