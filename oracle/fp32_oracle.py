@@ -39,7 +39,7 @@ PERTURBATIONS = ("kchunk", "zcols", "bhn_outside", "stale_h1", "tile_rootv",    
 
 
 def units_per_cta(H):
-    """U of csrc/decoder_common.cuh pick_U: CTA c owns hidden units c*U .. c*U+U-1 of every gate block."""
+    """U of csrc/library.cuh units_per_cta: CTA c owns hidden units c*U .. c*U+U-1 of every gate block."""
     return 4 if H % 4 == 0 and H // 4 <= 132 else 8
 
 

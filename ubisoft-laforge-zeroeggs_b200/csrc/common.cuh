@@ -148,6 +148,28 @@ __host__ __device__ inline V3 quat_from_helical_bwd(V3 h, Q4 dE) {
 __device__ __forceinline__ float elu_f(float x) { return x > 0.0f ? x : expm1f(x); }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// GRU cell of one (unit, sample) in nn.GRU's gate order r, z, n (b_hn inside r * (.)): gi_* / gh_* are the input- and hidden-side
+// pre-activations.  Writes the gates, returns h = (1 - z) n + z h_prev.  The FMA is explicit: left to contraction, which of the two
+// products gets fused would depend on where the caller loads h_prev.
+__device__ __forceinline__ float gru_gate_fwd(float gi_r, float gi_z, float gi_n, float gh_r, float gh_z, float gh_n, float h_prev,
+                                              float& r, float& z, float& n) {
+  r = sigmoid_f(gi_r + gh_r);
+  z = sigmoid_f(gi_z + gh_z);
+  n = tanhf(gi_n + r * gh_n);
+  return fmaf(1.f - z, n, z * h_prev);
+}
+
+// its backward: returns dgi (r,z,n), dgh (r,z,n) and dh*z
+__device__ __forceinline__ void gru_gate_bwd(float dh, float r, float z, float n, float ghn, float hprev,
+                                             float (&dgi)[3], float (&dgh)[3], float& dhz) {
+  float dn = dh * (1.f - z), dz = dh * (hprev - n);
+  dhz = dh * z;
+  float dpn = dn * (1.f - n * n), dpz = dz * z * (1.f - z);
+  float dpr = dpn * ghn * r * (1.f - r);
+  dgi[0] = dpr; dgi[1] = dpz; dgi[2] = dpn;
+  dgh[0] = dpr; dgh[1] = dpz; dgh[2] = dpn * r;
+}
+
 // ------------------------------------------------------------------ async copy / cache-controlled access
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   unsigned s = (unsigned)__cvta_generic_to_shared(smem);
@@ -159,45 +181,40 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 __device__ __forceinline__ float ld_cg(const float* p) { return __ldcg(p); }
 
-// ------------------------------------------------------------------ grid-wide barrier for persistent kernels
-// All CTAs of a cooperative launch call grid_sync() the same number of times.  `bar` points at two
-// zero-initialised unsigned ints in global memory: [0] arrival counter (monotone), [1] error flag.
-// A bounded spin (~2 s) turns a would-be hang into an error flag + early exit.
-struct GridBarrier {
-  unsigned* counter;
-  unsigned* error;
-  unsigned epoch;
-  unsigned nblocks;
-};
-
+// ------------------------------------------------------------------ grid-wide barriers for persistent kernels
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
 
-// returns false on timeout / peer error (caller must unwind: every CTA sees the flag)
-__device__ __forceinline__ bool grid_sync(GridBarrier& gb) {
-  __shared__ int s_ok;
+// spins until the arrival counter reaches `target`; a barrier that has not completed after ~2 s traps, so the launch fails with a
+// CUDA error instead of hanging or returning partial results
+__device__ __forceinline__ void grid_wait(const unsigned* counter, unsigned target) {
+  long long t0 = clock64();
+  while (ld_acquire_u32(counter) < target) {
+    if (clock64() - t0 > 4000000000LL) __trap();
+  }
+}
+
+// All CTAs of a cooperative launch call grid_sync() the same number of times.  `bar` points at a zero-initialised arrival counter
+// (monotone) in global memory.
+struct GridBarrier {
+  unsigned* counter;
+  unsigned epoch;
+  unsigned nblocks;
+  __device__ explicit GridBarrier(unsigned* bar) : counter(bar), epoch(0), nblocks(gridDim.x) {}
+};
+
+__device__ __forceinline__ void grid_sync(GridBarrier& gb) {
   __syncthreads();
   gb.epoch += 1;
   if (threadIdx.x == 0) {
-    int ok = 1;
     __threadfence();
     atomicAdd(gb.counter, 1u);
-    const unsigned target = gb.epoch * gb.nblocks;
-    long long t0 = clock64();
-    unsigned it = 0;
-    while (ld_acquire_u32(gb.counter) < target) {
-      if ((++it & 1023u) == 0) {
-        if (ld_acquire_u32(gb.error) != 0u) { ok = 0; break; }
-        if (clock64() - t0 > 4000000000LL) { atomicExch(gb.error, 1u); ok = 0; break; }
-      }
-    }
-    s_ok = ok;
+    grid_wait(gb.counter, gb.epoch * gb.nblocks);
   }
   __syncthreads();
-  return s_ok != 0;
 }
 
 }  // namespace zeggs

@@ -81,7 +81,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
   const int c = blockIdx.x, tid = threadIdx.x, warp = tid >> 5;
   const int H = a.H, T = a.T, nbt = g.nbt;
   float* wstage = stage + warp * 2 * SkinnyCfg<RTM>::STG;
-  GridBarrier gb; gb.counter = bw.bar; gb.error = bw.bar + 1; gb.epoch = 0; gb.nblocks = gridDim.x;
+  GridBarrier gb(bw.bar);
   const float* PB1 = d.packed + (size_t)c * K1P * bg.R1;
   const float* PB2 = d.packed + bg.off2 + (size_t)c * 3 * H * 2 * U;    // + p * 3H * 2V per pass
   const float* PB3a = d.packed + bg.off3a + (size_t)c * 3 * H * 2 * U;
@@ -178,7 +178,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
     for (int tile = 0; tile < bg.n4b; ++tile) phase_R(T - 1, bt, tile, false);
     phase_R_root(T - 1, bt, false);
   }
-  if (!grid_sync(gb)) return;
+  grid_sync(gb);
 
   for (int t = T - 1; t >= 1; --t) {
     if constexpr (FILM) {
@@ -205,7 +205,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
         }
         __syncthreads();
       }
-      if (!grid_sync(gb)) return;
+      grid_sync(gb);
     }
     // ------------------------------------------------------------ B1 (FiLM: B1b)
     for (int bt = 0; bt < nbt; ++bt)
@@ -239,7 +239,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
       }
       __syncthreads();
     }
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     // ------------------------------------------------------------ B2
     for (int bt = 0; bt < nbt; ++bt)
     for (int p = 0; p < NP; ++p) {
@@ -270,7 +270,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
       }
       __syncthreads();
     }
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     // ------------------------------------------------------------ B3
     for (int bt = 0; bt < nbt; ++bt) {
       for (int p = 0; p < NP; ++p) {
@@ -319,7 +319,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
       }
     }
     if (t == 1) break;
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     // ------------------------------------------------------------ B4 + R(t-1)
     for (int bt = 0; bt < nbt; ++bt) {
       const float* x = bw.DPA + t * actH + (size_t)bt * H * 32;
@@ -333,7 +333,7 @@ decoder_bwd_kernel(zeggs_decoder_fwd_args a, DecGeom g, BwdGeom bg, DecWs w, Bwd
       }
       phase_R_root(t - 1, bt, true);
     }
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
   }
 }
 
@@ -444,11 +444,12 @@ __global__ void elu_bwd_kernel(float* __restrict__ dx, const float* __restrict__
   if (i < n) { float v = y[i]; dx[i] *= (v > 0.f ? 1.f : v + 1.f); }
 }
 
-__global__ void colsum_kernel(const float* __restrict__ x, int rows, int cols, float* __restrict__ out) {
+// out[c] = sum over rows of x[r][c] (row stride ld)
+__global__ void colsum_ld_kernel(const float* __restrict__ x, int rows, int cols, int ld, float* __restrict__ out) {
   int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= cols) return;
   float s = 0.f;
-  for (int r = 0; r < rows; ++r) s += x[(size_t)r * cols + c];
+  for (int r = 0; r < rows; ++r) s += x[(size_t)r * ld + c];
   out[c] = s;
 }
 
@@ -616,15 +617,15 @@ int cse_backward(const zeggs_decoder_fwd_args& a, const zeggs_decoder_bwd_args& 
   cse_gather_kernel<<<ceil_div(a.B * 2 * H, 256), 256, 0, stream>>>(a.B, H, bw.DH0, bw.DH1, bw.cse_dout);
   count_launch();
   r = sgemm_launch(1, 2 * H, H, a.B, bw.cse_dout, 2 * H, w.cse_h2, H, nullptr, b.dWc2, H, 0, 0, stream); if (r) return r;
-  colsum_kernel<<<ceil_div(2 * H, 256), 256, 0, stream>>>(bw.cse_dout, a.B, 2 * H, b.dbc2); count_launch();
+  colsum_ld_kernel<<<ceil_div(2 * H, 256), 256, 0, stream>>>(bw.cse_dout, a.B, 2 * H, 2 * H, b.dbc2); count_launch();
   r = gemm_f32_auto(2, a.B, H, 2 * H, bw.cse_dout, 2 * H, a.Wc2, H, nullptr, bw.cse_d2, H, 0, 0, stream); if (r) return r;
   elu_bwd_kernel<<<ceil_div(a.B * H, 256), 256, 0, stream>>>(bw.cse_d2, w.cse_h2, (size_t)a.B * H); count_launch();
   r = sgemm_launch(1, H, H, a.B, bw.cse_d2, H, w.cse_h1, H, nullptr, b.dWc1, H, 0, 0, stream); if (r) return r;
-  colsum_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d2, a.B, H, b.dbc1); count_launch();
+  colsum_ld_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d2, a.B, H, H, b.dbc1); count_launch();
   r = gemm_f32_auto(2, a.B, H, H, bw.cse_d2, H, a.Wc1, H, nullptr, bw.cse_d1, H, 0, 0, stream); if (r) return r;
   elu_bwd_kernel<<<ceil_div(a.B * H, 256), 256, 0, stream>>>(bw.cse_d1, w.cse_h1, (size_t)a.B * H); count_launch();
   r = sgemm_launch(1, H, Kin, a.B, bw.cse_d1, H, w.cse_in, Kin, nullptr, b.dWc0, Kin, 0, 0, stream); if (r) return r;
-  colsum_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d1, a.B, H, b.dbc0); count_launch();
+  colsum_ld_kernel<<<ceil_div(H, 256), 256, 0, stream>>>(bw.cse_d1, a.B, H, H, b.dbc0); count_launch();
   r = gemm_f32_auto(2, a.B, Kin, H, bw.cse_d1, H, a.Wc0, Kin, nullptr, bw.cse_din, Kin, 0, 0, stream); if (r) return r;
   ZCHECK_LAUNCH();
   return ZEGGS_OK;
@@ -749,15 +750,6 @@ __global__ void pack_film_bwd_kernel(DecGeom g, int R1, const float* __restrict_
     const int r = i % R1P, k = (i / R1P) % H, cp = i / ((size_t)R1P * H);   // cp = c * (U / V) + p
     out[i] = r < V ? Wm[(size_t)k * H + cp * V + r] : 0.f;
   }
-}
-
-// out[c] = sum over rows of x[r][c] (row stride ld)
-__global__ void colsum_ld_kernel(const float* __restrict__ x, int rows, int cols, int ld, float* __restrict__ out) {
-  int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= cols) return;
-  float s = 0.f;
-  for (int r = 0; r < rows; ++r) s += x[(size_t)r * ld + c];
-  out[c] = s;
 }
 
 // dStyle[b][0][:] += the CellStateEncoder's input gradient of the style columns (frame 0 has no FiLM term)

@@ -62,17 +62,6 @@ struct BwdArgsDev {
   const float* packed;
 };
 
-// GRU gate backward for one (unit, sample): returns dgi (r,z,n), dgh (r,z,n) and dh*z
-__device__ __forceinline__ void gru_gate_bwd(float dh, float r, float z, float n, float ghn, float hprev,
-                                             float (&dgi)[3], float (&dgh)[3], float& dhz) {
-  float dn = dh * (1.f - z), dz = dh * (hprev - n);
-  dhz = dh * z;
-  float dpn = dn * (1.f - n * n), dpz = dz * z * (1.f - z);
-  float dpr = dpn * ghn * r * (1.f - r);
-  dgi[0] = dpr; dgi[1] = dpz; dgi[2] = dpn;
-  dgh[0] = dpr; dgh[1] = dpz; dgh[2] = dpn * r;
-}
-
 // ------------------------------------------------------------------ host steps shared by the two backward routines
 // Weight gradients (slots t = 1..T-1) on the tensor cores: each of the 11 fp32 histories is re-laid out once as bf16 hi (and lo)
 // [rows][T*nbt*32] (contraction index contiguous) from the base of the scratch buffer, all hi parts first, then all lo parts.  (ld * 2)

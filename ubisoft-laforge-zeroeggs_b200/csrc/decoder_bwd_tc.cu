@@ -126,17 +126,6 @@ inline BtWs make_btws(void* base, const DecGeom& g) {
 // trace of CTAs 0 and 1 (both ranks of pair 0): dbg[c][reverse step < 64][event < 32], clock64 of the CTA's SM
 #define BTDBG(ev) do { if (iw.dbg && c < 2 && lane == 0 && (T - 1 - t) < 64) iw.dbg[c * 2048 + (T - 1 - t) * 32 + (ev)] = clock64(); } while (0)
 
-// store U bf16 values at (row, k = j0..j0+U-1) of an image with `rows`-row tiles
-template <int U>
-__device__ __forceinline__ void store_img_row(uint8_t* img, int rows, int row, int j0, const float (&h)[U]) {
-  __nv_bfloat16 t[U];
-#pragma unroll
-  for (int i = 0; i < U; ++i) t[i] = __float2bfloat16_rn(h[i]);
-  uint8_t* p = img + img_off(rows, row, j0);
-  if (U == 8) *reinterpret_cast<uint4*>(p) = *reinterpret_cast<const uint4*>(t);
-  else *reinterpret_cast<uint2*>(p) = *reinterpret_cast<const uint2*>(t);
-}
-
 // Warp roles (224 threads): warps 0..3 = the MMA warpgroup, warp 4 = epilogue (lane = sample), warp 5 = weight producer (runs
 // ahead across barriers), warp 6 = activation loader (grid-barrier waiter; streams the rank's half of the A images through the
 // ring).  A chain's accumulator D[64 x N] is one m64 wgmma accumulator in the warpgroup's registers; once the chain has completed

@@ -1,39 +1,21 @@
 // Geometry, workspace layout and the weight-stationary "skinny GEMM" building block shared by the
 // decoder forward and backward persistent kernels.
 #pragma once
-#include <type_traits>
 #include "library.cuh"
 
 namespace zeggs {
 
 constexpr int K1P = 1136;  // P_IN (1134) rounded up to the 16-row k-chunk
 
-// units per CTA: the grid G = H/U must fit one CTA per SM (132 on the H100 SXM).  At U = 16 the fp32 recurrences run each stage as
-// two passes of 8 units (pass_units), so the register tiles and shared-memory stages stay those of U = 8.
-inline int pick_U(int H) {
-  if (H % 4 == 0 && H / 4 <= 132) return 4;
-  if (H % 8 == 0 && H / 8 <= 132) return 8;
-  if (H % 16 == 0 && H / 16 <= 132) return 16;
-  return -1;
-}
-
-// calls f(std::integral_constant<int, U>{}) for the units per CTA pick_U chose (4, 8 or 16): the one place a run-time U becomes the
-// template argument of the fp32 kernels
-template <class F>
-auto dispatch_units(int U, F&& f) {
-  if (U == 4) return f(std::integral_constant<int, 4>{});
-  if (U == 8) return f(std::integral_constant<int, 8>{});
-  return f(std::integral_constant<int, 16>{});
-}
-
-// units of one pass of the fp32 recurrences: a CTA's U units are U / pass_units(U) passes, each with its own contiguous weight slice
+// units of one pass of the fp32 recurrences: a CTA's U units are U / pass_units(U) passes, each with its own contiguous weight slice.
+// At U = 16 each stage runs as two passes of 8 units, so the register tiles and shared-memory stages stay those of U = 8.
 __host__ __device__ constexpr int pass_units(int U) { return U < 8 ? U : 8; }
 
 // hidden sizes the tensor-core recurrence (engine 1: forward and BPTT kernels) covers; every tc size / pack / run entry point
 // applies this one rule (the BPTT kernel pairs 64-wide k-blocks, and below 384 nothing has been validated)
 inline bool tc_hidden_ok(int H) { return H % 128 == 0 && H >= 384 && H <= 1024; }
 // hidden sizes the fp32 recurrences (engine 0, normal and FiLM) cover: every fp32 size / pack / run entry point applies this rule
-inline bool fp32_hidden_ok(int H) { return H % 16 == 0 && pick_U(H) > 0; }
+inline bool fp32_hidden_ok(int H) { return H % 16 == 0 && units_per_cta(H) > 0; }
 
 struct DecGeom {
   int B, H, S, Z, A;   // A = 1134 + S + Z
@@ -50,7 +32,7 @@ struct DecGeom {
 inline DecGeom make_geom(int B, int H, int S, int Z) {
   DecGeom g;
   g.B = B; g.H = H; g.S = S; g.Z = Z; g.A = P_IN + S + Z;
-  g.U = pick_U(H); g.G = H / g.U;
+  g.U = units_per_cta(H); g.G = H / g.U;
   g.nbt = ceil_div(B, 32);
   g.rpc = ceil_div(P_OUT, g.G);
   g.n4t = ceil_div(g.rpc, 16);

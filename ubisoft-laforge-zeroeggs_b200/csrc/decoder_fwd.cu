@@ -157,7 +157,7 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
   const int c = blockIdx.x, tid = threadIdx.x, warp = tid >> 5;
   const int H = a.H, T = a.T, nbt = g.nbt;
   float* wstage = stage + warp * 2 * SkinnyCfg<RT2>::STG;
-  GridBarrier gb; gb.counter = w.bar; gb.error = w.bar + 1; gb.epoch = 0; gb.nblocks = gridDim.x;
+  GridBarrier gb(w.bar);
 
   const float* P1 = a.packed + (size_t)c * K1P * 4 * U;
   const float* P2 = a.packed + g.off_p2() + (size_t)c * H * 6 * U;
@@ -197,7 +197,7 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
       }
       __syncthreads();
     }
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     // ------------------------------------------------------------ stage 2 (GRU layer 0)
     for (int q = 0; q < nbt * NP; ++q) {
       const int bt = q / NP, p = q % NP;
@@ -215,10 +215,8 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
         float ghr = red_sum<6 * V>(red, 3 * V + v, b) + a.b_hh0[0 * H + j];
         float ghz = red_sum<6 * V>(red, 4 * V + v, b) + a.b_hh0[1 * H + j];
         float ghn = red_sum<6 * V>(red, 5 * V + v, b) + a.b_hh0[2 * H + j];
-        float r = sigmoid_f(gir + ghr), z = sigmoid_f(giz + ghz);
-        float n = tanhf(gin + r * ghn);
-        float hp = ld_cg(xb + (size_t)j * 32 + b);
-        float h = (1.f - z) * n + z * hp;
+        float r, z, n;
+        float h = gru_gate_fwd(gir, giz, gin, ghr, ghz, ghn, ld_cg(xb + (size_t)j * 32 + b), r, z, n);
         w.H0[ts * actH + ((size_t)bt * H + j) * 32 + b] = h;
         if (w.save) {
           float* G = w.G0 + ((size_t)t * nbt + bt) * 4 * H * 32;
@@ -228,7 +226,7 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
       }
       __syncthreads();
     }
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     // ------------------------------------------------------------ stage 3 (GRU layer 1)
     for (int q = 0; q < nbt * NP; ++q) {
       const int bt = q / NP, p = q % NP;
@@ -246,10 +244,8 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
         float ghr = red_sum<6 * V>(red, 3 * V + v, b) + a.b_hh1[0 * H + j];
         float ghz = red_sum<6 * V>(red, 4 * V + v, b) + a.b_hh1[1 * H + j];
         float ghn = red_sum<6 * V>(red, 5 * V + v, b) + a.b_hh1[2 * H + j];
-        float r = sigmoid_f(gir + ghr), z = sigmoid_f(giz + ghz);
-        float n = tanhf(gin + r * ghn);
-        float hp = ld_cg(xb + (size_t)j * 32 + b);
-        float h = (1.f - z) * n + z * hp;
+        float r, z, n;
+        float h = gru_gate_fwd(gir, giz, gin, ghr, ghz, ghn, ld_cg(xb + (size_t)j * 32 + b), r, z, n);
         w.H1[ts * actH + ((size_t)bt * H + j) * 32 + b] = h;
         if (w.save) {
           float* G = w.G1 + ((size_t)t * nbt + bt) * 4 * H * 32;
@@ -259,7 +255,7 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
       }
       __syncthreads();
     }
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     if constexpr (FILM) {
       // ---------------------------------------------------------- stage 3b (FiLM layer2: c = ELU(Wm h1 + bm) * g[H:] + be[H:])
       for (int q = 0; q < nbt * NP; ++q) {
@@ -278,7 +274,7 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
         }
         __syncthreads();
       }
-      if (!grid_sync(gb)) return;
+      grid_sync(gb);
     }
     // ------------------------------------------------------------ stage 4 (layer2 -- FiLM: layer3 -- + pose integration)
     for (int bt = 0; bt < nbt; ++bt) {
@@ -329,7 +325,7 @@ __global__ void __launch_bounds__(256, 1) decoder_fwd_kernel(zeggs_decoder_fwd_a
       }
       __syncthreads();
     }
-    if (t + 1 < T) { if (!grid_sync(gb)) return; }
+    if (t + 1 < T) grid_sync(gb);
   }
 }
 
@@ -347,7 +343,7 @@ static int check_fwd_args(const zeggs_decoder_fwd_args* a) {
   ZCHECK_ARG(fp32_hidden_ok(a->H), "decoder: hidden size %d unsupported (need H%%16==0, H<=2112)", a->H);
   ZCHECK_ARG(a->S >= 1 && a->Z >= 1 && a->S + a->Z <= 256, "decoder: bad S=%d Z=%d", a->S, a->Z);
   if (a->engine != 1) {
-    const int U = pick_U(a->H);
+    const int U = units_per_cta(a->H);
     auto smem_of = [U](int nbt) { return dispatch_units(U, [nbt](auto u) { return fwd_smem_bytes<u>(nbt); }); };
     const int nbt = ceil_div(a->B, 32);
     DeviceLimits lim;

@@ -479,7 +479,7 @@ decoder_fwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, TcGeom tg, DecWs w, T
         for (int u = 0; u < U; ++u) av[u] = sv[u] > 0.f ? sv[u] : __expf(sv[u]) - 1.0f;   // ELU (modules.py:183)
 #pragma unroll
         for (int i = 0; i < 3 * U; ++i) gi0p[i] = sv[U + i];
-        if (act) store_img_units<U>(tw.ab, b, j0, av);
+        if (act) store_img_row<U>(tw.ab, 32, b, j0, av);
         TCDBG(6);
         grid_arrive(w.bar);                     // only the bf16 image feeds other CTAs: publish it first ...
         TCDBG(7);
@@ -522,7 +522,7 @@ decoder_fwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, TcGeom tg, DecWs w, T
             hv[u] = (1.f - zz[u]) * nn[u] + zz[u] * hp[u];
           }
         }
-        if (act) store_img_units<U>(tw.h0b[t & 1], b, j0, hv);
+        if (act) store_img_row<U>(tw.h0b[t & 1], 32, b, j0, hv);
         TCDBG(13);
         grid_arrive(w.bar);
         if (act) {
@@ -562,7 +562,7 @@ decoder_fwd_tc_kernel(zeggs_decoder_fwd_args a, DecGeom g, TcGeom tg, DecWs w, T
             hv[u] = (1.f - zz[u]) * nn[u] + zz[u] * hp[u];
           }
         }
-        if (act) store_img_units<U>(tw.h1b[t & 1], b, j0, hv);
+        if (act) store_img_row<U>(tw.h1b[t & 1], 32, b, j0, hv);
         TCDBG(18);
         grid_arrive(w.bar);
         TCDBG(19);

@@ -528,7 +528,7 @@ extern "C" int zeggs_style_enc_gru_fwd(const zeggs_style_enc_gru_args* ap, void*
   const bool vae = a.mu != nullptr;
   ZCHECK_ARG(B >= 1 && T >= 1 && Cin >= 1 && E >= 1 && (!vae || E % 2 == 0) && a.x && a.z && (a.logvar != nullptr) == vae,
              "style_enc_gru: bad arguments");
-  ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru: hidden size %d unsupported (H %% 4 == 0 and H <= 528, H %% 8 == 0 and H <= 1056, "
+  ZCHECK_ARG(units_per_cta(H) > 0, "style_enc_gru: hidden size %d unsupported (H %% 4 == 0 and H <= 528, H %% 8 == 0 and H <= 1056, "
              "or H %% 16 == 0 and H <= 2112)", H);
   ZCHECK_ARG(B <= style_gru_max_batch(H), "style_enc_gru: batch %d too large: at hidden size %d the backward's shared memory holds at "
              "most %d samples per call", B, H, style_gru_max_batch(H));
@@ -558,7 +558,7 @@ extern "C" int zeggs_style_enc_gru_bwd(const zeggs_style_enc_gru_args* ap, const
   const int B = a.B, T = a.T, Cin = a.C_in, H = a.H, E = a.E, M = B * T;
   const bool vae = a.mu != nullptr;
   ZCHECK_ARG(vae || (g.dz && !g.dmu && !g.dlogvar), "style_enc_gru bwd: without the VAE (mu == NULL) dz [B,E] is required and dmu / dlogvar must be NULL");
-  ZCHECK_ARG(style_gru_units(H) > 0, "style_enc_gru bwd: hidden size %d unsupported", H);
+  ZCHECK_ARG(units_per_cta(H) > 0, "style_enc_gru bwd: hidden size %d unsupported", H);
   ZCHECK_ARG(B <= style_gru_max_batch(H), "style_enc_gru bwd: batch %d too large: at hidden size %d the shared memory holds at most %d "
              "samples per call", B, H, style_gru_max_batch(H));
   StyleGruWs w = style_gru_ws(a.workspace, B, T, Cin, H, E, vae);

@@ -1,6 +1,7 @@
 // The library's internal host API: launch bookkeeping, per-device launch limits, the persistent-kernel launcher, workspace
 // carving, the GEMM front end and the launchers one source offers the others.
 #pragma once
+#include <type_traits>
 #include <utility>
 #include "common.cuh"
 #include "../../include/zeggs_b200.h"
@@ -50,6 +51,25 @@ int launch_persistent(void (*kernel)(P...), int grid, int block, size_t smem, in
   ZCHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...));
   count_launch();
   return ZEGGS_OK;
+}
+
+// ------------------------------------------------------------------ the fp32 recurrences' partition (decoder and GRU style encoder)
+// units per CTA: CTA c owns hidden units c*U .. c*U+U-1, and the grid G = H/U must fit one CTA per SM (132 on the H100 SXM).  4 up to
+// H = 528, 8 up to 1056, 16 up to 2112; -1 = H unsupported.
+inline int units_per_cta(int H) {
+  if (H % 4 == 0 && H / 4 <= 132) return 4;
+  if (H % 8 == 0 && H / 8 <= 132) return 8;
+  if (H % 16 == 0 && H / 16 <= 132) return 16;
+  return -1;
+}
+
+// calls f(std::integral_constant<int, U>{}) for the units per CTA units_per_cta chose (4, 8 or 16): the one place a run-time U becomes
+// the template argument of the fp32 kernels
+template <class F>
+auto dispatch_units(int U, F&& f) {
+  if (U == 4) return f(std::integral_constant<int, 4>{});
+  if (U == 8) return f(std::integral_constant<int, 8>{});
+  return f(std::integral_constant<int, 16>{});
 }
 
 // the largest number of 32-sample batch tiles whose dynamic shared memory smem_of(nbt) (growing with nbt) fits `cap` bytes
@@ -111,7 +131,6 @@ int sgemm_batched2_launch(int mode, int M, int N, int K, const float* A, int lda
                           long long sA, long long sB, long long sC, int inner, long long iA, long long iB, long long iC,
                           float alpha, cudaStream_t stream);
 // StyleEncoderGRU recurrences (style_gru.cu)
-int style_gru_units(int H);
 int style_gru_max_batch(int H);
 int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
                          unsigned* bar, cudaStream_t s);

@@ -95,14 +95,6 @@ __device__ __forceinline__ void gru_stage_cols16(float* __restrict__ dst, const 
   }
 }
 
-// units per CTA: 4 while the grid fits one CTA per SM of the H100 (H <= 528), else 8 (H <= 1056), else 16 (H <= 2112); 0 = unsupported
-int style_gru_units(int H) {
-  if (H % 4 == 0 && H / 4 <= 132) return 4;
-  if (H % 8 == 0 && H / 8 <= 132) return 8;
-  if (H % 16 == 0 && H / 16 <= 132) return 16;
-  return 0;
-}
-
 // dynamic shared memory per CTA: the forward kernel's with nbt = 0, the BPTT kernel's with its nbt 32-sample tiles of carry.
 // U = 16 keeps no weights resident: the forward holds one [KC][GRU_WS] chunk of W_hh rows, the BPTT one [KC][U] chunk of columns.
 template <int U>
@@ -119,12 +111,10 @@ constexpr size_t GRU_SMEM_LIMIT = 232448;
 
 // the largest batch one call takes at hidden size H (0 = H unsupported): the BPTT kernel's carry grows by U*32 floats per tile
 int style_gru_max_batch(int H) {
-  const int U = style_gru_units(H);
-  if (U == 0) return 0;
-  auto bytes = [&](int nbt) { return U == 4 ? gru_smem_bytes<4>(H, nbt) : U == 8 ? gru_smem_bytes<8>(H, nbt) : gru_smem_bytes<16>(H, nbt); };
-  int nbt = 0;
-  while (bytes(nbt + 1) <= GRU_SMEM_LIMIT) ++nbt;
-  return 32 * nbt;
+  const int U = units_per_cta(H);
+  if (U < 0) return 0;
+  auto smem_of = [U, H](int nbt) { return dispatch_units(U, [H, nbt](auto u) { return gru_smem_bytes<u>(H, nbt); }); };
+  return 32 * max_batch_tiles(smem_of, GRU_SMEM_LIMIT);
 }
 
 // ------------------------------------------------------------------ forward recurrence (modules.py:341, nn.GRU gate order r, z, n)
@@ -148,7 +138,7 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_fwd_kernel(int B, int T, i
       const int r = i / H, k = i - r * H, g = r / U, u = r - g * U;
       Ws[(size_t)k * R + r] = Whh[(size_t)(g * H + c * U + u) * H + k];
     }
-  GridBarrier gb; gb.counter = bar; gb.error = bar + 1; gb.epoch = 0; gb.nblocks = gridDim.x;
+  GridBarrier gb(bar);
   const int H3 = 3 * H;
   for (int t = 0; t < T; ++t) {
     const float* hprev = Hs + (size_t)t * B * H;
@@ -191,17 +181,15 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_fwd_kernel(int B, int T, i
           gh[g] = s + bhh[g * H + j];
         }
         const float* gi = GI + ((size_t)b * T + t) * H3;
-        const float r = sigmoid_f(gi[j] + gh[0]), z = sigmoid_f(gi[H + j] + gh[1]);
-        const float n = tanhf(gi[2 * H + j] + r * gh[2]);
-        const float hp = __ldcg(hprev + (size_t)b * H + j);
-        const float h = (1.f - z) * n + z * hp;
+        float r, z, n;
+        const float h = gru_gate_fwd(gi[j], gi[H + j], gi[2 * H + j], gh[0], gh[1], gh[2], __ldcg(hprev + (size_t)b * H + j), r, z, n);
         Hs[((size_t)(t + 1) * B + b) * H + j] = h;
         float* G = Gs + ((size_t)t * B + b) * 4 * H;
         G[j] = r; G[H + j] = z; G[2 * H + j] = n; G[3 * H + j] = gh[2];
         if (t == T - 1) hcat[(size_t)b * 2 * H + j] = h;
       }
     }
-    if (t + 1 < T) { if (!grid_sync(gb)) return; }
+    if (t + 1 < T) grid_sync(gb);
   }
 }
 
@@ -231,27 +219,23 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_bwd_kernel(int B, int T, i
     carry[i] = b < B ? dhf[(size_t)b * ld_dhf + c * U + u] : 0.f;
   }
   __syncthreads();
-  GridBarrier gb; gb.counter = bar; gb.error = bar + 1; gb.epoch = 0; gb.nblocks = gridDim.x;
+  GridBarrier gb(bar);
   for (int t = T - 1; t >= 0; --t) {
     // phase A: gate gradients of the own units (h(t) = (1-z) n + z h(t-1))
     for (int i = tid; i < nbt * U * 32; i += GRU_THREADS) {
       const int bt = i / (U * 32), u = (i >> 5) % U, bl = i & 31, b = bt * 32 + bl, j = c * U + u;
       if (b >= B) continue;
-      const float dh = carry[i];
       const float* G = Gs + ((size_t)t * B + b) * 4 * H;
-      const float r = G[j], z = G[H + j], n = G[2 * H + j], ghn = G[3 * H + j];
-      const float hp = Hs[((size_t)t * B + b) * H + j];
-      const float dpn = dh * (1.f - z) * (1.f - n * n);
-      const float dpr = dpn * ghn * r * (1.f - r);
-      const float dpz = dh * (hp - n) * z * (1.f - z);
+      float dgi[3], dgh[3], dhz;
+      gru_gate_bwd(carry[i], G[j], G[H + j], G[2 * H + j], G[3 * H + j], Hs[((size_t)t * B + b) * H + j], dgi, dgh, dhz);
       float* gi = dGih + ((size_t)b * T + t) * H3;
-      gi[j] = dpr; gi[H + j] = dpz; gi[2 * H + j] = dpn;
+      gi[j] = dgi[0]; gi[H + j] = dgi[1]; gi[2 * H + j] = dgi[2];
       float* gh = dGhh + ((size_t)t * B + b) * H3;
-      gh[j] = dpr; gh[H + j] = dpz; gh[2 * H + j] = dpn * r;
-      carry[i] = dh * z;
+      gh[j] = dgh[0]; gh[H + j] = dgh[1]; gh[2 * H + j] = dgh[2];
+      carry[i] = dhz;
     }
     if (t == 0) break;                     // h(-1) = 0 is a constant: no dh(-1)
-    if (!grid_sync(gb)) return;
+    grid_sync(gb);
     // phase B: dh(t-1)[own units] += dG_hh(t) W_hh[:, own units]
     const float* dg = dGhh + (size_t)t * B * H3;
     for (int bt = 0; bt < nbt; ++bt) {
@@ -296,14 +280,15 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) gru_bwd_kernel(int B, int T, i
 
 // ------------------------------------------------------------------ the reverse direction: one GRU cell from h = 0
 // GIr [B][3H] = x[:, T-1] W_ih_r^T + b_ih_r;  W_hh_r h = 0, so the hidden-side pre-activations are b_hh_r.  h_r -> hcat[:, H:2H].
+// Both kernels pass h_prev = -0, not +0: x + (-0) is x and -0 - n is -n for every x and n, signs of zero included, so the cell's
+// (1 - z) n + z h_prev and its dh (h_prev - n) are exactly (1 - z) n and -dh n.
 __global__ void rev_cell_fwd_kernel(int B, int H, const float* __restrict__ GIr, const float* __restrict__ bhh, float* __restrict__ hcat) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * H) return;
   const int b = i / H, j = i - b * H;
   const float* gi = GIr + (size_t)b * 3 * H;
-  const float r = sigmoid_f(gi[j] + bhh[j]), z = sigmoid_f(gi[H + j] + bhh[H + j]);
-  const float n = tanhf(gi[2 * H + j] + r * bhh[2 * H + j]);
-  hcat[(size_t)b * 2 * H + H + j] = (1.f - z) * n;
+  float r, z, n;
+  hcat[(size_t)b * 2 * H + H + j] = gru_gate_fwd(gi[j], gi[H + j], gi[2 * H + j], bhh[j], bhh[H + j], bhh[2 * H + j], -0.f, r, z, n);
 }
 // dh_r = dhcat[:, H:2H] -> dGIr (input-side pre-activations) and dGHr (hidden-side: b_hh_r's gradient rows)
 __global__ void rev_cell_bwd_kernel(int B, int H, const float* __restrict__ GIr, const float* __restrict__ bhh, const float* __restrict__ dhcat,
@@ -312,44 +297,40 @@ __global__ void rev_cell_bwd_kernel(int B, int H, const float* __restrict__ GIr,
   if (i >= B * H) return;
   const int b = i / H, j = i - b * H;
   const float* gi = GIr + (size_t)b * 3 * H;
-  const float r = sigmoid_f(gi[j] + bhh[j]), z = sigmoid_f(gi[H + j] + bhh[H + j]);
-  const float n = tanhf(gi[2 * H + j] + r * bhh[2 * H + j]);
-  const float dh = dhcat[(size_t)b * 2 * H + H + j];
-  const float dpn = dh * (1.f - z) * (1.f - n * n);
-  const float dpr = dpn * bhh[2 * H + j] * r * (1.f - r);
-  const float dpz = -dh * n * z * (1.f - z);
+  float r, z, n, dgi[3], dgh[3], dhz;
+  gru_gate_fwd(gi[j], gi[H + j], gi[2 * H + j], bhh[j], bhh[H + j], bhh[2 * H + j], -0.f, r, z, n);
+  gru_gate_bwd(dhcat[(size_t)b * 2 * H + H + j], r, z, n, bhh[2 * H + j], -0.f, dgi, dgh, dhz);
   float* a = dGIr + (size_t)b * 3 * H;
   float* h = dGHr + (size_t)b * 3 * H;
-  a[j] = dpr; a[H + j] = dpz; a[2 * H + j] = dpn;
-  h[j] = dpr; h[H + j] = dpz; h[2 * H + j] = dpn * r;
+  a[j] = dgi[0]; a[H + j] = dgi[1]; a[2 * H + j] = dgi[2];
+  h[j] = dgh[0]; h[H + j] = dgh[1]; h[2 * H + j] = dgh[2];
 }
 
 // ------------------------------------------------------------------ host side
 int style_gru_fwd_launch(int B, int T, int H, const float* Whh, const float* bhh, const float* GI, float* Hs, float* Gs, float* hcat,
                          unsigned* bar, cudaStream_t s) {
-  const int U = style_gru_units(H);
+  const int U = units_per_cta(H);
   ZCHECK_ARG(U > 0 && B >= 1 && T >= 1, "style GRU: hidden size %d unsupported (need H %% 4 == 0, H <= 528, H %% 8 == 0, H <= 1056, "
              "or H %% 16 == 0, H <= 2112)", H);
   ZCHECK_CUDA(cudaMemsetAsync(bar, 0, 2 * sizeof(unsigned), s));
   ZCHECK_CUDA(cudaMemsetAsync(Hs, 0, (size_t)B * H * sizeof(float), s));     // h(-1) = 0
-  if (U == 4) return launch_persistent(gru_fwd_kernel<4>, H / 4, GRU_THREADS, gru_smem_bytes<4>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
-  if (U == 8) return launch_persistent(gru_fwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
-  return launch_persistent(gru_fwd_kernel<16>, H / 16, GRU_THREADS, gru_smem_bytes<16>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
+  return dispatch_units(U, [&](auto u) {
+    return launch_persistent(gru_fwd_kernel<u>, H / u, GRU_THREADS, gru_smem_bytes<u>(H, 0), 1, s, B, T, H, Whh, bhh, GI, Hs, Gs, hcat, bar);
+  });
 }
 
 int style_gru_bwd_launch(int B, int T, int H, const float* Whh, const float* Hs, const float* Gs, const float* dhf, int ld_dhf,
                          float* dGih, float* dGhh, unsigned* bar, cudaStream_t s) {
-  const int U = style_gru_units(H);
+  const int U = units_per_cta(H);
   ZCHECK_ARG(U > 0 && B >= 1 && T >= 1, "style GRU: hidden size %d unsupported", H);
   ZCHECK_ARG(B <= style_gru_max_batch(H), "style GRU bwd: batch %d above the %d samples the shared memory holds at hidden size %d", B,
              style_gru_max_batch(H), H);
   ZCHECK_CUDA(cudaMemsetAsync(bar, 0, 2 * sizeof(unsigned), s));
   const int nbt = (B + 31) / 32;
-  if (U == 4)
-    return launch_persistent(gru_bwd_kernel<4>, H / 4, GRU_THREADS, gru_smem_bytes<4>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
-  if (U == 8)
-    return launch_persistent(gru_bwd_kernel<8>, H / 8, GRU_THREADS, gru_smem_bytes<8>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
-  return launch_persistent(gru_bwd_kernel<16>, H / 16, GRU_THREADS, gru_smem_bytes<16>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih, dGhh, bar);
+  return dispatch_units(U, [&](auto u) {
+    return launch_persistent(gru_bwd_kernel<u>, H / u, GRU_THREADS, gru_smem_bytes<u>(H, nbt), 1, s, B, T, H, Whh, Hs, Gs, dhf, ld_dhf, dGih,
+                             dGhh, bar);
+  });
 }
 
 int style_gru_rev_cell_fwd(int B, int H, const float* GIr, const float* bhh, float* hcat, cudaStream_t s) {

@@ -77,25 +77,19 @@ __device__ __forceinline__ void acc_ld(const float* p, int ld, float (&v)[NC]) {
 __device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 __device__ __forceinline__ float fast_tanh(float x) { return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * x)); }
 
-// grid barrier split in two halves: the epilogue warp arrives, the activation loader waits
+// grid barrier split in two halves: the epilogue warp arrives, the activation loader waits (grid_wait, common.cuh)
 __device__ __forceinline__ void grid_arrive(unsigned* counter) {
   __syncwarp();   // the lanes' stores happen-before lane 0's release (cumulative at gpu scope)
   if ((threadIdx.x & 31) == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;\n" ::"l"(counter) : "memory");
 }
-__device__ __forceinline__ void grid_wait(const unsigned* counter, unsigned target) {
-  long long t0 = clock64();
-  while (ld_acquire_u32(counter) < target) {
-    if (clock64() - t0 > 4000000000LL) __trap();
-  }
-}
 
-// write U consecutive bf16 values (units j0..j0+U-1 of sample row b) into an activation image
+// store U bf16 values at (row, k = j0..j0+U-1) of an image with `rows`-row tiles
 template <int U>
-__device__ __forceinline__ void store_img_units(uint8_t* img, int b, int j0, const float (&h)[U]) {
+__device__ __forceinline__ void store_img_row(uint8_t* img, int rows, int row, int j0, const float (&h)[U]) {
   __nv_bfloat16 t[U];
 #pragma unroll
   for (int i = 0; i < U; ++i) t[i] = __float2bfloat16_rn(h[i]);
-  uint8_t* p = img + img_off(32, b, j0);
+  uint8_t* p = img + img_off(rows, row, j0);
   if (U == 8) *reinterpret_cast<uint4*>(p) = *reinterpret_cast<const uint4*>(t);
   else *reinterpret_cast<uint2*>(p) = *reinterpret_cast<const uint2*>(t);
 }
