@@ -6,7 +6,9 @@
 // Parallel form of the recursive filters: the gating-block boundaries cut every clip into SEGMENTS (1600 samples at 16 kHz);
 // one thread owns one (clip, segment), starts `warm` samples earlier from a zero state (K-weighting's slowest pole pair, the
 // 38 Hz double pole, decays as n r^n with r = 0.985: 4800 samples reduce the start-up transient below 1e-28) and accumulates
-// the energy of its segment; a second kernel folds segments into blocks and applies the two gates.  Samples may be float32
+// the energy of its segment; a second kernel, one CTA per clip, applies the two gates.  Each gating pass recomputes every block
+// energy z_j from the handful of segment energies the block covers (4 at 16 kHz), in a fixed order, so the meter keeps no
+// per-block array and takes clips of any length; the result is deterministic.  Samples may be float32
 // or int16 PCM (x / 32768, audio_files.py:211-236).  The gain is applied by the mel kernel at load (mel.cu), not here:
 // the waveform is never rewritten in HBM.
 #include "library.cuh"
@@ -52,23 +54,22 @@ __global__ void __launch_bounds__(128) kweight_segment_energy_kernel(const TIn* 
 __global__ void __launch_bounds__(128) loudness_gate_kernel(const double* __restrict__ seg_energy, int n_seg, const int* __restrict__ blk_lo,
                                                             const int* __restrict__ blk_hi, int n_blocks, double inv_block_len, double target,
                                                             float* __restrict__ gain_out, float* __restrict__ lufs_out) {
-  extern __shared__ double zs[];                // [n_blocks]
   __shared__ double red[128];
   __shared__ int redn[128];
   const int clip = blockIdx.x, tid = threadIdx.x;
   const double* se = seg_energy + (size_t)clip * n_seg;
-  for (int j = tid; j < n_blocks; j += blockDim.x) {
+  auto block_energy = [&](int j) -> double {                  // z_j = (sum of its segments' energies) / (0.4 s * rate)
     double s = 0.0;
-    for (int k = blk_lo[j]; k < blk_hi[j]; ++k) s += se[k];
-    zs[j] = s * inv_block_len;
-  }
-  __syncthreads();
+    for (int k = __ldg(blk_lo + j); k < __ldg(blk_hi + j); ++k) s += se[k];
+    return s * inv_block_len;
+  };
   auto gated_mean = [&](double thr, bool strict) -> double {     // mean of z_j over blocks with l_j (>= | >) thr; NaN if none
     double s = 0.0; int c = 0;
     for (int j = tid; j < n_blocks; j += blockDim.x) {
-      const double l = -0.691 + 10.0 * log10(zs[j]);
+      const double z = block_energy(j);
+      const double l = -0.691 + 10.0 * log10(z);
       const bool in = strict ? (l > thr && l > -70.0) : (l >= thr);
-      if (in) { s += zs[j]; ++c; }
+      if (in) { s += z; ++c; }
     }
     red[tid] = s; redn[tid] = c;
     __syncthreads();
@@ -96,7 +97,8 @@ extern "C" int zeggs_loudness_gain(const zeggs_loudness_args* ap, void* stream_)
   ZCHECK_ARG(ap, "loudness: null args");
   const zeggs_loudness_args& a = *ap;
   cudaStream_t s = (cudaStream_t)stream_;
-  ZCHECK_ARG(a.n_clips >= 0 && a.n_samples >= 1 && a.n_seg >= 1 && a.n_blocks >= 1 && a.n_blocks <= 6000, "loudness: bad shape");
+  ZCHECK_ARG(a.n_clips >= 0 && a.n_samples >= 1 && a.n_seg >= 1 && a.n_blocks >= 1, "loudness: bad shape");
+  ZCHECK_ARG((long long)a.n_clips * a.n_seg + 127 <= INT_MAX, "loudness: too many (clip, segment) pairs for one grid");   // int thread index
   ZCHECK_ARG((a.wav != nullptr) != (a.wav_i16 != nullptr), "loudness: exactly one of wav / wav_i16");
   ZCHECK_ARG(a.seg_bounds && a.blk_seg_lo && a.blk_seg_hi && a.gain_out && a.workspace, "loudness: null table/output pointer");
   ZCHECK_ARG(a.workspace_bytes >= zeggs_loudness_workspace_bytes(a.n_clips, a.n_seg), "loudness: workspace too small");
@@ -108,8 +110,8 @@ extern "C" int zeggs_loudness_gain(const zeggs_loudness_args* ap, void* stream_)
   if (a.wav) kweight_segment_energy_kernel<float><<<ceil_div(total, 128), 128, 0, s>>>(a.wav, a.n_clips, a.n_samples, q, a.seg_bounds, a.n_seg, a.warm, se);
   else kweight_segment_energy_kernel<short><<<ceil_div(total, 128), 128, 0, s>>>(a.wav_i16, a.n_clips, a.n_samples, q, a.seg_bounds, a.n_seg, a.warm, se);
   count_launch();
-  loudness_gate_kernel<<<a.n_clips, 128, (size_t)a.n_blocks * sizeof(double), s>>>(se, a.n_seg, a.blk_seg_lo, a.blk_seg_hi, a.n_blocks, a.inv_block_len,
-                                                                                    a.target_lufs, a.gain_out, a.lufs_out);
+  loudness_gate_kernel<<<a.n_clips, 128, 0, s>>>(se, a.n_seg, a.blk_seg_lo, a.blk_seg_hi, a.n_blocks, a.inv_block_len, a.target_lufs,
+                                                 a.gain_out, a.lufs_out);
   count_launch();
   ZCHECK_LAUNCH();
   return ZEGGS_OK;
