@@ -519,6 +519,58 @@ typedef struct {
 } zeggs_resample_args;
 int zeggs_resample(const zeggs_resample_args* a, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * BVH MOTION block text on the device (zeggs_b200.animation.load_bvh, zeggs_b200.bvhio.save_bvh; the reference's anim/bvh.py:load
+ * and :save).  The HIERARCHY header stays on the host.
+ *
+ * Parser.  text [n_bytes] is everything after the "Frame Time:" line.  Lines are split at "\r\n", "\r" and "\n" (what Python's
+ * universal-newline read followed by split("\n") gives), lines that are empty after strip() are dropped and the first n_frames of the
+ * rest are the rows; tokens are split on the ASCII whitespace of str.split().  A token on the exact fast path (see bvh_text.cuh:
+ * [+-]?(digits[.digits]|.digits)([eE][+-]?digits)?, at most 2^53 as an integer of its significant digits, decimal exponent within
+ * +-22) is written to out [n_frames, C] as float() would parse it, bit for bit; any other token is not parsed: its (row * C + column,
+ * byte offset in text) pair goes to flagged [max_flagged][2] for the caller to fill.  status [3] (device, written by the call):
+ *   status[0] rows taken = min(n_frames, non-blank lines), status[1] flagged tokens (entries past max_flagged are not stored),
+ *   status[2] bit 0: a row's token count is not C (out is incomplete), bit 1: a byte >= 0x80 (Unicode is the host's business).
+ * n_bytes < 2^31.
+ */
+typedef struct {
+  long long n_bytes;
+  int n_frames, C, max_flagged;
+  const unsigned char* text;
+  double* out;
+  long long* flagged;
+  int* status;
+  void* workspace;
+  size_t workspace_bytes;
+} zeggs_bvh_parse_args;
+size_t zeggs_bvh_parse_motion_workspace_size(long long n_bytes, int n_frames);
+int zeggs_bvh_parse_motion(const zeggs_bvh_parse_args* a, void* stream);
+
+/* Writer: the MOTION rows of the reference writer, byte for byte.  Row t is, for c in 0 .. C-1 with C = 3 + 3 J, "%f " of the float64
+ * value of column c, then "\n"; columns 0..2 are positions[t][0][0..2] and columns 3 + 3 i + k are rotations[t][seq[i]][k] (seq [J]
+ * int32, the depth-first joint order).  positions / rotations [T,J,3] are float32 (in_f64 = 0) or float64 (in_f64 = 1).
+ * out [out_capacity] receives the text (out_capacity >= zeggs_bvh_format_motion_max_size(T, J)); row_start [T+1] the byte offset of
+ * every row and, at T, the total length.  A value whose "%f" does not fit the 128-bit path (|v| >= 2^128 / 10^6) is written as
+ * nothing and its index t * C + c goes to flagged [max_flagged]: the caller formats those rows itself.
+ * status [2] (device, written by the call): status[0] total bytes, status[1] flagged values (entries past max_flagged are not stored).
+ */
+typedef struct {
+  int T, J, in_f64, max_flagged;
+  const void* positions;
+  const void* rotations;
+  const int* seq;
+  char* out;
+  long long out_capacity;
+  long long* row_start;
+  long long* flagged;
+  long long* status;
+  void* workspace;
+  size_t workspace_bytes;
+} zeggs_bvh_format_args;
+long long zeggs_bvh_format_motion_max_size(int T, int J);
+size_t zeggs_bvh_format_motion_workspace_size(int T, int J);
+int zeggs_bvh_format_motion(const zeggs_bvh_format_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -118,6 +118,13 @@ MomentsArgs = _struct("MomentsArgs", ints=("n_groups",),
 ResampleArgs = _struct("ResampleArgs", tail=[("n_in", C.c_longlong), ("n_out", C.c_longlong), ("channels", C.c_int), ("dtype", C.c_int),
                                              ("L", C.c_int), ("M", C.c_int), ("K4", C.c_int), ("delay", C.c_longlong), ("pcm", C.c_void_p),
                                              ("taps", C.c_void_p), ("out", C.c_void_p)])
+BvhParseArgs = _struct("BvhParseArgs", tail=[("n_bytes", C.c_longlong), ("n_frames", C.c_int), ("C", C.c_int), ("max_flagged", C.c_int),
+                                             ("text", C.c_void_p), ("out", C.c_void_p), ("flagged", C.c_void_p), ("status", C.c_void_p),
+                                             ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
+BvhFormatArgs = _struct("BvhFormatArgs", ints=("T", "J", "in_f64", "max_flagged"),
+                        tail=[("positions", C.c_void_p), ("rotations", C.c_void_p), ("seq", C.c_void_p), ("out", C.c_void_p),
+                              ("out_capacity", C.c_longlong), ("row_start", C.c_void_p), ("flagged", C.c_void_p), ("status", C.c_void_p),
+                              ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
 
 
 # every symbol include/zeggs_b200.h declares: (name, restype, argtypes)
@@ -130,7 +137,8 @@ def struct_mirrors():
             "zeggs_style_enc_gru_args": StyleEncGruArgs, "zeggs_style_enc_gru_grads": StyleEncGruGrads,
             "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs,
             "zeggs_resample_args": ResampleArgs, "zeggs_decoder_film_fwd_args": DecoderFilmFwdArgs,
-            "zeggs_decoder_film_bwd_args": DecoderFilmBwdArgs}
+            "zeggs_decoder_film_bwd_args": DecoderFilmBwdArgs, "zeggs_bvh_parse_args": BvhParseArgs,
+            "zeggs_bvh_format_args": BvhFormatArgs}
 
 
 SYMBOLS = [
@@ -201,6 +209,11 @@ SYMBOLS = [
     ("zeggs_masked_moments_workspace_bytes", C.c_size_t, [C.c_longlong, C.c_int]),
     ("zeggs_masked_moments", C.c_int, [C.POINTER(MomentsArgs), C.c_void_p]),
     ("zeggs_resample", C.c_int, [C.POINTER(ResampleArgs), C.c_void_p]),
+    ("zeggs_bvh_parse_motion_workspace_size", C.c_size_t, [C.c_longlong, C.c_int]),
+    ("zeggs_bvh_parse_motion", C.c_int, [C.POINTER(BvhParseArgs), C.c_void_p]),
+    ("zeggs_bvh_format_motion_max_size", C.c_longlong, [C.c_int, C.c_int]),
+    ("zeggs_bvh_format_motion_workspace_size", C.c_size_t, [C.c_int, C.c_int]),
+    ("zeggs_bvh_format_motion", C.c_int, [C.POINTER(BvhFormatArgs), C.c_void_p]),
 ]
 
 _lib = None

@@ -1,4 +1,4 @@
-"""BVH in, pose features out: the host-side data-format edge in front of the accelerated path (numpy, not a kernel).
+"""BVH in, pose features out: the data-format edge in front of the accelerated path (numpy; the MOTION numbers parse on the device).
 
 Mirrors what the reference does to a style example / first-pose BVH before the networks see it:
   ZEGGS/anim/bvh.py:4-134        load(): HIERARCHY + MOTION text -> rotations (degrees, file channel order), positions, offsets, ...
@@ -18,16 +18,30 @@ _CHAN = {"Xrotation": "x", "Yrotation": "y", "Zrotation": "z"}
 
 # ---------------------------------------------------------------------------------------------- BVH text
 def load_bvh(path):
-    """-> dict(rotations [T,J,3] deg, positions [T,J,3], offsets [J,3], parents [J], names, order, frametime), like bvh.py:load."""
+    """-> dict(rotations [T,J,3] deg, positions [T,J,3], offsets [J,3], parents [J], names, order, frametime), like bvh.py:load.
+    The MOTION block is parsed on the device when the library and a CUDA device are available (bit-identical to the host parse, which
+    decides every case the device parser leaves to it), on the host otherwise."""
+    got = _load_bvh_device(path) if _device_parse_available() else None
+    if got is not None:
+        header, data = got
+        return _assemble(path, header, data)
+    with open(path, "r") as f:
+        lines = iter(f.read().split("\n"))
+    header = _parse_header(lines)
+    nframes = header[-1]
+    rows = [r for r in lines if r.strip()]
+    data = np.array([np.array(r.split(), dtype=np.float64) for r in rows[:nframes]]) if nframes else np.zeros((0, 0))
+    return _assemble(path, header, data)
+
+
+def _parse_header(lines):
+    """HIERARCHY of a BVH file from an iterator over its lines; consumes them up to the "Frame Time:" line.
+    -> (names, offsets, parents, chans, order, frametime, nframes)"""
     names, offsets, parents, chans = [], [], [], []
     stack, order, frametime, nframes = [], None, None, None
     in_end = False
-    with open(path, "r") as f:
-        lines = f.read().split("\n")
-    k = 0
-    while k < len(lines):
-        ln = lines[k].strip()
-        k += 1
+    for line in lines:
+        ln = line.strip()
         if not ln or ln == "HIERARCHY":
             continue
         tok = ln.split()
@@ -55,9 +69,13 @@ def load_bvh(path):
         elif tok[0] == "Frame" and tok[1] == "Time:":
             frametime = float(tok[2])
             break
+    return names, offsets, parents, chans, order, frametime, nframes
+
+
+def _assemble(path, header, data):
+    """MOTION values data [T, C] (float64, file channel order) + header -> the load_bvh dict."""
+    names, offsets, parents, chans, order, frametime, _ = header
     J = len(names)
-    rows = [r for r in lines[k:] if r.strip()]
-    data = np.array([np.array(r.split(), dtype=np.float64) for r in rows[:nframes]]) if nframes else np.zeros((0, 0))
     T = data.shape[0]
     off = np.asarray(offsets, dtype=np.float64)
     positions = np.repeat(off[None], T, axis=0)
@@ -75,6 +93,89 @@ def load_bvh(path):
         col += n
     return dict(rotations=rotations.astype(np.float32), positions=positions.astype(np.float32), offsets=off.astype(np.float32),
                 parents=np.asarray(parents, dtype=np.int32), names=names, order=order or "zyx", frametime=frametime)
+
+
+# MOTION tokens the device leaves to the host (not on the exact fast path) are filled here one by one; with more than this many, the
+# whole block is parsed on the host
+MAX_FLAGGED_TOKENS = 1 << 16
+_LINE_BREAK = re.compile(rb"\r\n|\r|\n")
+_TOKEN = re.compile(rb"[^ \t\n\r\x0b\x0c\x1c-\x1f]+")
+
+
+def _device_parse_available():
+    import torch
+    from . import _lib
+    if not torch.cuda.is_available():
+        return False
+    try:
+        _lib.lib()
+    except _lib.ZeggsError:
+        return False
+    return True
+
+
+def _header_lines(buf, state):
+    """The lines of an ASCII file as Python's universal-newline read + split("\\n") gives them; state["next"] = where the text after
+    the last line handed out starts.  A non-ASCII byte raises UnicodeDecodeError."""
+    pos = 0
+    for m in _LINE_BREAK.finditer(buf):
+        state["next"] = m.end()
+        yield buf[pos:m.start()].tobytes().decode("ascii")
+        pos = m.end()
+    state["next"] = len(buf)
+    yield buf[pos:].tobytes().decode("ascii")
+
+
+def _load_bvh_device(path):
+    """-> (header, data [T, C] float64) with the MOTION block parsed by zeggs_bvh_parse_motion, or None when the host parser must
+    decide: non-ASCII text, no frames, a joint with other than 3 or 6 channels, a block of 2 GB or more, no rows, a row whose token
+    count is not C, a token numpy rejects, or more tokens off the fast path than MAX_FLAGGED_TOKENS."""
+    import ctypes as C
+    import os
+    import torch
+    from . import _lib
+    n = os.path.getsize(path)
+    host = torch.empty(n, dtype=torch.uint8, pin_memory=True)
+    buf = host.numpy()
+    with open(path, "rb") as f:
+        if f.readinto(memoryview(buf)) != n:
+            return None
+    state = {}
+    try:
+        header = _parse_header(_header_lines(memoryview(buf), state))
+    except UnicodeDecodeError:
+        return None
+    chans, frametime, nframes = header[3], header[5], header[6]
+    if frametime is None or not nframes or nframes < 0 or not chans or any(c not in (3, 6) for c in chans):
+        return None
+    start, ncol = state["next"], sum(chans)
+    if n - start >= 1 << 31:
+        return None
+    dev = torch.device("cuda", torch.cuda.current_device())
+    text = torch.empty(n - start, dtype=torch.uint8, device=dev)
+    text.copy_(host[start:], non_blocking=True)
+    out = torch.empty((nframes, ncol), dtype=torch.float64, device=dev)
+    flagged = torch.empty((MAX_FLAGGED_TOKENS, 2), dtype=torch.int64, device=dev)
+    status = torch.empty(3, dtype=torch.int32, device=dev)
+    l = _lib.lib()
+    ws = torch.empty(int(l.zeggs_bvh_parse_motion_workspace_size(n - start, nframes)), dtype=torch.uint8, device=dev)
+    a = _lib.BvhParseArgs(n_bytes=n - start, n_frames=nframes, C=ncol, max_flagged=MAX_FLAGGED_TOKENS, text=text.data_ptr(),
+                          out=out.data_ptr(), flagged=flagged.data_ptr(), status=status.data_ptr(), workspace=ws.data_ptr(),
+                          workspace_bytes=ws.numel())
+    _lib.check(l.zeggs_bvh_parse_motion(C.byref(a), _lib.stream_ptr()), "zeggs_bvh_parse_motion")
+    rows, nflag, bad = (int(v) for v in status.cpu())
+    if bad or rows == 0 or nflag > MAX_FLAGGED_TOKENS:
+        return None
+    data = out[:rows].cpu().numpy()
+    if nflag:
+        block, flat = memoryview(buf)[start:], data.reshape(-1)
+        for idx, off in flagged[:nflag].cpu().numpy():
+            tok = _TOKEN.match(block, int(off)).group().decode("ascii")
+            try:
+                flat[idx] = np.array([tok], dtype=np.float64)[0]           # the host parse's own conversion of this token
+            except ValueError:
+                return None
+    return header, data
 
 
 # ---------------------------------------------------------------------------------------------- quaternions (w first)

@@ -202,8 +202,8 @@ def data_pipeline(conf, label_names=None, device="cuda"):
             if conf["save_trimmed_animation"]:
                 (out_dir / "trimmed" / folder).mkdir(parents=True, exist_ok=True)
                 centre_root_in_place(pos, rot, anim["order"])
-                bvhio.save_bvh(out_dir / "trimmed" / folder / (stem + ".bvh"), pos, rot, anim["parents"], names, anim["order"],
-                               anim["frametime"], offsets=anim["offsets"])
+                bvhio.save_bvh(out_dir / "trimmed" / folder / (stem + ".bvh"), torch.from_numpy(pos).to(dev), torch.from_numpy(rot).to(dev),
+                               anim["parents"], names, anim["order"], anim["frametime"], offsets=anim["offsets"])
             nframes = len(rot)
             wav_in = wav_dev if wav_dev.dtype == torch.int16 else wav_dev.to(torch.float32)
             feats = audio.preprocess_audio(wav_in, anim_fps, nframes, aconf, feature_type, device=dev)

@@ -204,7 +204,7 @@ def generate_gesture(audio_file, styles, network_path, data_path, results_path, 
                               f("anim_input_mean"), f("anim_input_std"), f("anim_output_mean"), f("anim_output_std"), float(dt))
         V = dict(zip(POSE_KEYS, out))
         pos, eul = ops.pose_to_bvh_channels(V["root_pos"], V["root_rot"], V["lpos"], V["ltxy"], (0.0, 0.0, 0.0), (1.0, 0.0, 0.0, 0.0))
-        pos, eul = pos[0].cpu().numpy(), eul[0].cpu().numpy()
+        pos, eul = pos[0], eul[0]                                                        # formatted as BVH text on the device
     if file_name is None:
         file_name = f"audio_{Path(audio_file).stem}_label_{anim_name}"
     try:

@@ -364,7 +364,6 @@ def write_samples(samples_dir, iteration, ds, se, de, st, stats, details, style_
                 V = dict(zip(POSE_KEYS, V))
                 pos, eul = ops.pose_to_bvh_channels(*[torch.cat([c[k], V[k]], 0) for k in ("root_pos", "root_rot", "lpos", "ltxy")],
                                                     rebase=False)
-                pos, eul = pos.cpu().numpy(), eul.cpu().numpy()
                 lab = details["label_names"][label]
                 try:
                     for j, kind in enumerate(("ground", "predict")):
