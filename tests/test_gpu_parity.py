@@ -1,9 +1,8 @@
-"""GPU parity: the CUDA path (through the C ABI) against the CPU oracle and the committed reference goldens.
+"""GPU parity: the CUDA path (through the C ABI) against the CPU oracle and the committed reference goldens.  The GEMM front end has its
+own float64 tests: tests/test_gemm_f64_gpu.py.
 
 Tolerances (stated per SURVEY.md 8d):
   mel features            abs <= 2e-4 on the ln-domain 80-mel + energy features (fp32 FFT vs the f64 reference)
-  sgemm (fp32 SIMT)       rel <= 2e-5 of max|C|
-  tc_gemm bf16            equals fp32 matmul of the bf16-rounded operands to 1e-5 rel; split-bf16 (x3) <= 2e-5 rel
   decoder fp32 path       against the float64 oracle, the bounds of oracle/fp32_oracle.py: per-pose-channel max-abs
                           <= FP32_FWD_TOL * max(1, max|ref|) (de-normalised units), free-running; gradients max-abs
                           <= FP32_GEMM_GRAD_TOL * max|ref| (GEMM mode 1); reference goldens (fp32) 2e-4
@@ -25,44 +24,6 @@ def dev():
         pytest.skip("needs a CUDA device")
     ensure_built()
     return torch.device("cuda:0")
-
-
-# ---------------------------------------------------------------------------------------------- GEMMs
-@pytest.mark.parametrize("M,N,K", [(7, 5, 3), (64, 64, 16), (130, 257, 1198), (32, 2048, 1024), (384, 32, 384), (200, 17, 100)])
-def test_sgemm(dev, M, N, K):
-    from zeggs_b200 import ops
-    g = torch.Generator().manual_seed(M * 1000 + N)
-    A = torch.randn(M, K, generator=g)
-    B = torch.randn(N, K, generator=g)
-    bias = torch.randn(N, generator=g)
-    ref = torch.nn.functional.elu(A.double() @ B.double().T + bias.double())
-    got = ops.sgemm(A.to(dev), B.to(dev), bias.to(dev), act=1)
-    err, sc = report(f"sgemm nt {M}x{N}x{K}", got, ref)
-    assert err <= 2e-5 * max(sc, 1.0)
-    At = torch.randn(K, M, generator=g)
-    Bt = torch.randn(K, N, generator=g)
-    got = ops.sgemm(At.to(dev), Bt.to(dev), trans_a=True)
-    err, sc = report(f"sgemm tn {M}x{N}x{K}", got, At.double().T @ Bt.double())
-    assert err <= 2e-5 * max(sc, 1.0)
-
-
-@pytest.mark.parametrize("M,N,K", [(128, 128, 64), (128, 128, 256), (256, 384, 512), (200, 300, 1136), (3072, 2286, 1024), (1024, 1262, 4096), (130, 256, 192)])
-def test_tc_gemm_bf16(dev, M, N, K):
-    from zeggs_b200 import ops
-    g = torch.Generator().manual_seed(M + N + K)
-    A = torch.randn(M, K, generator=g).to(dev)
-    B = torch.randn(N, K, generator=g).to(dev)
-    Ah, Al = ops.split_bf16(A)
-    Bh, Bl = ops.split_bf16(B)
-    assert torch.equal(Ah[:, :K], A.to(torch.bfloat16))
-    got1 = ops.tc_gemm(Ah, Bh, K=K)
-    ref1 = Ah[:, :K].double() @ Bh[:, :K].double().T
-    err, sc = report(f"tc_gemm bf16 {M}x{N}x{K}", got1, ref1)
-    assert err <= 1e-5 * sc
-    got3 = ops.tc_gemm(Ah, Bh, Al, Bl, K=K)
-    ref3 = A.double() @ B.double().T
-    err, sc = report(f"tc_gemm bf16x3 {M}x{N}x{K}", got3, ref3)
-    assert err <= 2e-5 * sc
 
 
 def test_normalize_rows_is_bit_identical_to_the_two_tensor_ops(dev):
@@ -386,67 +347,6 @@ def test_fused_radam_vs_reference_golden(dev, golden_dir):
         p.grad.copy_(torch.from_numpy(g["grads"][i]).to(dev))
         opt.step()
         assert np.abs(p.detach().cpu().numpy() - g["traj"][i]).max() <= 2e-7, i
-
-
-@pytest.mark.parametrize("mode,M,N,K", [(0, 300, 200, 1000), (1, 512, 3402, 1536), (2, 700, 260, 129), (0, 12288 // 8, 512, 3402),
-                                        (0, 32, 512, 3402), (1, 128, 384, 12288), (2, 32, 1198, 2048), (1, 64, 64, 12288)])   # last four: split-K
-def test_gemm_f32_front_end_tcgen05(dev, mode, M, N, K):
-    """fp32 in/out GEMM through tensor-core split-bf16 (default mode 1): <= 4e-5 relative to max|C| vs float64 (K up to 3402)."""
-    from zeggs_b200 import _lib, ops
-    ops.ensure_scratch(dev)
-    g = torch.Generator().manual_seed(mode * 7 + M)
-    if mode == 0:
-        A, B = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g); ref = A.double() @ B.double().T
-    elif mode == 1:
-        A, B = torch.randn(K, M, generator=g), torch.randn(K, N, generator=g); ref = A.double().T @ B.double()
-    else:
-        A, B = torch.randn(M, K, generator=g), torch.randn(K, N, generator=g); ref = A.double() @ B.double()
-    Ad, Bd = A.to(dev), B.to(dev)
-    out = torch.empty(M, N, device=dev)
-    _lib.check(_lib.lib().zeggs_gemm_f32_ctx(ops.ctx_ptr(dev), mode, M, N, K, Ad.data_ptr(), Ad.stride(0), Bd.data_ptr(), Bd.stride(0), None,
-                                             out.data_ptr(), N, 0, 0, _lib.stream_ptr()), "zeggs_gemm_f32_ctx")
-    err, sc = report(f"gemm_f32 mode{mode} {M}x{N}x{K}", out, ref)
-    assert err <= 4e-5 * sc
-
-
-def test_gemm_f32_splitk_epilogue(dev):
-    """split-K path (few output tiles, long K): bias + ELU + accumulate are applied once, by the reduction kernel."""
-    from zeggs_b200 import _lib, ops
-    ops.ensure_scratch(dev)
-    g = torch.Generator().manual_seed(5)
-    M, N, K = 32, 300, 4096
-    A, B, bias, C0 = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g), torch.randn(N, generator=g), torch.randn(M, N, generator=g)
-    ref = C0.double() + torch.nn.functional.elu(A.double() @ B.double().T + bias.double())
-    Ad, Bd, bd, out = A.to(dev), B.to(dev), bias.to(dev), C0.to(dev).clone()
-    _lib.check(_lib.lib().zeggs_gemm_f32_ctx(ops.ctx_ptr(dev), 0, M, N, K, Ad.data_ptr(), K, Bd.data_ptr(), K, bd.data_ptr(), out.data_ptr(), N, 1, 1,
-                                             _lib.stream_ptr()), "zeggs_gemm_f32_ctx")
-    err, sc = report("gemm_f32 split-K bias+elu+accumulate", out, ref)
-    assert err <= 4e-5 * sc
-
-
-@pytest.mark.parametrize("M,N,K", [(32, 300, 4096), (256, 700, 384)])        # split-K (few output tiles, long K) / not split
-@pytest.mark.parametrize("mode", [0, 1, 2])
-def test_gemm_f32_epilogue_every_operand_layout(dev, mode, M, N, K):
-    """bias + ELU + accumulate epilogue of the split-bf16 GEMM front end in every operand layout (mode 0: A[M,K] B[N,K]^T -- the tc
-    engine's hoisted cond terms --, 1: A[K,M]^T B[K,N] -- its fold matrix --, 2: A[M,K] B[K,N]), with and without split-K: <= 4e-5
-    relative to max|C| vs float64.  The call carries its own zeggs_ctx (GEMM mode 1, fast_wgrad off), so the result does not depend on
-    which decoder engine the process has selected: with the tensor-core engine the shared context runs mode-1 products as ONE bf16 pass."""
-    import ctypes as C
-    from zeggs_b200 import _lib
-    scratch = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    ctx = _lib.Ctx(scratch=scratch.data_ptr(), scratch_bytes=scratch.numel(), gemm_mode=1, fast_wgrad=0)
-    g = torch.Generator().manual_seed(5 + mode)
-    A = torch.randn(K, M, generator=g) if mode == 1 else torch.randn(M, K, generator=g)
-    B = torch.randn(N, K, generator=g) if mode == 0 else torch.randn(K, N, generator=g)
-    bias, C0 = torch.randn(N, generator=g), torch.randn(M, N, generator=g)
-    prod = A.double().T if mode == 1 else A.double()
-    prod = prod @ (B.double().T if mode == 0 else B.double())
-    ref = C0.double() + torch.nn.functional.elu(prod + bias.double())
-    Ad, Bd, bd, out = A.to(dev), B.to(dev), bias.to(dev), C0.to(dev).clone()
-    _lib.check(_lib.lib().zeggs_gemm_f32_ctx(C.addressof(ctx), mode, M, N, K, Ad.data_ptr(), Ad.stride(0), Bd.data_ptr(), Bd.stride(0),
-                                             bd.data_ptr(), out.data_ptr(), N, 1, 1, _lib.stream_ptr()), "zeggs_gemm_f32_ctx")
-    err, sc = report(f"gemm_f32 mode{mode} {M}x{N}x{K} bias+elu+accumulate", out, ref)
-    assert err <= 4e-5 * sc
 
 
 # ---------------------------------------------------------------------------------------------- inference path (config 1)

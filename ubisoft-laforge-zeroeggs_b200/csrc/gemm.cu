@@ -163,20 +163,27 @@ int sgemm_batched2_launch(int mode, int M, int N, int K, const float* A, int lda
                           long long sA, long long sB, long long sC, int inner, long long iA, long long iB, long long iC,
                           float alpha, cudaStream_t stream) {
   ZCHECK_ARG(M > 0 && N > 0 && K > 0 && A && B && C && batch >= 1 && batch <= 65535 && inner >= 1, "sgemm: bad arguments M=%d N=%d K=%d batch=%d", M, N, K, batch);
-  if (N <= 32 && mode != 0 && M >= 128) {
-    dim3 gridn(1, ceil_div(M, 128), batch);
-    if (mode == 1) sgemm_n32_kernel<1><<<gridn, 256, 0, stream>>>(M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
-    else sgemm_n32_kernel<2><<<gridn, 256, 0, stream>>>(M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
+  const bool n32 = N <= 32 && mode != 0 && M >= 128;
+  // grid.y holds at most 65535 row tiles: a taller product runs as consecutive row slices, one launch each (A and C offset by the
+  // slice's first row; in mode 1 a row of C is a column of A)
+  const int slice = 65535 * (n32 ? 128 : 64);
+  for (int m0 = 0; m0 < M; m0 += slice) {
+    const int Ms = std::min(slice, M - m0);
+    const float* As = A + (mode == 1 ? (size_t)m0 : (size_t)m0 * lda);
+    float* Cs = C + (size_t)m0 * ldc;
+    if (n32) {
+      dim3 gridn(1, ceil_div(Ms, 128), batch);
+      if (mode == 1) sgemm_n32_kernel<1><<<gridn, 256, 0, stream>>>(Ms, N, K, As, lda, B, ldb, bias, Cs, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
+      else sgemm_n32_kernel<2><<<gridn, 256, 0, stream>>>(Ms, N, K, As, lda, B, ldb, bias, Cs, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
+    } else {
+      dim3 grid(ceil_div(N, 64), ceil_div(Ms, 64), batch);
+      if (mode == 1) sgemm_kernel<1><<<grid, 256, 0, stream>>>(Ms, N, K, As, lda, B, ldb, bias, Cs, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
+      else if (mode == 2) sgemm_kernel<2><<<grid, 256, 0, stream>>>(Ms, N, K, As, lda, B, ldb, bias, Cs, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
+      else sgemm_kernel<0><<<grid, 256, 0, stream>>>(Ms, N, K, As, lda, B, ldb, bias, Cs, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
+    }
     count_launch();
     ZCHECK_LAUNCH();
-    return ZEGGS_OK;
   }
-  dim3 grid(ceil_div(N, 64), ceil_div(M, 64), batch);
-  if (mode == 1) sgemm_kernel<1><<<grid, 256, 0, stream>>>(M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
-  else if (mode == 2) sgemm_kernel<2><<<grid, 256, 0, stream>>>(M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
-  else sgemm_kernel<0><<<grid, 256, 0, stream>>>(M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, sA, sB, sC, inner, iA, iB, iC, alpha);
-  count_launch();
-  ZCHECK_LAUNCH();
   return ZEGGS_OK;
 }
 

@@ -31,7 +31,7 @@ template <int BN, int STAGES, bool FUSE>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K,
                const float* __restrict__ bias, float* __restrict__ C, int ldc, int act, int accumulate,
-               float* __restrict__ part, int kb_per_split) {
+               float* __restrict__ part, int kb_per_split, int mtile0) {
   constexpr int B_BYTES = BN * TG_BK * 2;
   constexpr int NOP = FUSE ? 2 : 1;                 // operand copies per stage (hi [, lo])
   constexpr int STAGE_A = NOP * TG_A_BYTES, STAGE_B = NOP * B_BYTES;
@@ -47,7 +47,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmMaps maps, int M, int N, int K,
 
   // warp index broadcast from lane 0: provably warp-uniform, so the role branches below do not count as divergent code for wgmma
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * TG_BM, n0 = blockIdx.x * BN;
+  const int m0 = (blockIdx.y + mtile0) * TG_BM, n0 = blockIdx.x * BN;
   // split-K: blockIdx.z owns k-blocks [kb0, kb0 + kblocks); its raw fp32 tile goes to part[z][M][N] (reduced afterwards)
   const int kb0 = blockIdx.z * kb_per_split;
   const int kblocks = min(kb_per_split, ceil_div(K, TG_BK) - kb0);
@@ -181,26 +181,33 @@ __global__ void split_bf16_kernel(const float* __restrict__ x, int rows, int col
   }
 }
 
-// transposing split: x[rows][cols] (ld_in) -> hi/lo [cols][ld_out] (ld_out >= rows, zero padded); 32x32 tiles
+// transposing split: x[rows][cols] (ld_in) -> hi/lo [cols][ld_out] (ld_out >= rows, zero padded); 32x32 tiles, blockIdx.y striding
+// over the ceil(ld_out / 32) row tiles (launch with split_t_grid)
 __global__ void split_bf16_t_kernel(const float* __restrict__ x, int rows, int cols, int ld_in,
                                     __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int ld_out) {
   __shared__ float tile[32][33];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += 8) {
-    const int r = r0 + i, c = c0 + threadIdx.x;
-    tile[i][threadIdx.x] = (r < rows && c < cols) ? x[(size_t)r * ld_in + c] : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += 8) {
-    const int c = c0 + i, r = r0 + threadIdx.x;     // output row c, output column r
-    if (c < cols && r < ld_out) {
-      const float v = tile[threadIdx.x][i];
-      const __nv_bfloat16 h = __float2bfloat16_rn(v);
-      hi[(size_t)c * ld_out + r] = h;
-      if (lo) lo[(size_t)c * ld_out + r] = __float2bfloat16_rn(v - __bfloat162float(h));
+  const int c0 = blockIdx.x * 32;
+  for (int r0 = blockIdx.y * 32; r0 < ld_out; r0 += gridDim.y * 32) {
+    for (int i = threadIdx.y; i < 32; i += 8) {
+      const int r = r0 + i, c = c0 + threadIdx.x;
+      tile[i][threadIdx.x] = (r < rows && c < cols) ? x[(size_t)r * ld_in + c] : 0.f;
     }
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += 8) {
+      const int c = c0 + i, r = r0 + threadIdx.x;     // output row c, output column r
+      if (c < cols && r < ld_out) {
+        const float v = tile[threadIdx.x][i];
+        const __nv_bfloat16 h = __float2bfloat16_rn(v);
+        hi[(size_t)c * ld_out + r] = h;
+        if (lo) lo[(size_t)c * ld_out + r] = __float2bfloat16_rn(v - __bfloat162float(h));
+      }
+    }
+    __syncthreads();
   }
 }
+
+// grid of split_bf16_t_kernel: one block per 32 x 32 tile up to grid.y's limit of 65535 row tiles (2,097,120 rows), striding beyond
+static dim3 split_t_grid(int cols, int ld_out) { return dim3(ceil_div(cols, 32), std::min(ceil_div(ld_out, 32), 65535)); }
 
 // k-major history [S][R_src][32] (slot stride given) -> hi/lo [R][S*32]: out[r][s*32 + b] = in[s][r][b].
 // One warp per history row r: lanes = samples b, the warp walks the slots (128 B in, 64 B out per slot, both streams
@@ -348,12 +355,16 @@ int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bf
   const int kbs = ceil_div(kblocks, splits);
   splits = ceil_div(kblocks, kbs);                        // every z gets at least one k-block
   float* const part = splits > 1 ? splitk_ws : nullptr;
-  const dim3 grid(ceil_div(N, BN), ceil_div(M, TG_BM), splits);
-  // with `part` set the kernel stores the raw tile and leaves bias, act and accumulate to the reduction
-  if (fused) tc_gemm_kernel<128, 3, true><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs);
-  else if (BN == 256) tc_gemm_kernel<256, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs);
-  else tc_gemm_kernel<128, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs);
-  count_launch();
+  // with `part` set the kernel stores the raw tile and leaves bias, act and accumulate to the reduction.  grid.y holds at most 65535
+  // row tiles: a taller product runs as consecutive slices of row tiles, one launch each, starting at row tile t0
+  const int mtiles = ceil_div(M, TG_BM);
+  for (int t0 = 0; t0 < mtiles; t0 += 65535) {
+    const dim3 grid(ceil_div(N, BN), std::min(mtiles - t0, 65535), splits);
+    if (fused) tc_gemm_kernel<128, 3, true><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs, t0);
+    else if (BN == 256) tc_gemm_kernel<256, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs, t0);
+    else tc_gemm_kernel<128, 4, false><<<grid, TG_THREADS, smem, stream>>>(maps, M, N, K, bias, C, ldc, act, accumulate, part, kbs, t0);
+    count_launch();
+  }
   if (part) {
     const size_t total = (size_t)M * N;
     splitk_reduce_kernel<<<(int)std::min<size_t>(1184, (total + 255) / 256), 256, 0, stream>>>(part, splits, M, N, bias, C, ldc, act, accumulate);
@@ -364,7 +375,7 @@ int tc_gemm_launch(int M, int N, int K, const __nv_bfloat16* A_hi, const __nv_bf
 }
 
 int split_t_launch(const float* x, int rows, int cols, int ld_in, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld_out, cudaStream_t stream) {
-  split_bf16_t_kernel<<<dim3(ceil_div(cols, 32), ceil_div(ld_out, 32)), dim3(32, 8), 0, stream>>>(x, rows, cols, ld_in, hi, lo, ld_out);
+  split_bf16_t_kernel<<<split_t_grid(cols, ld_out), dim3(32, 8), 0, stream>>>(x, rows, cols, ld_in, hi, lo, ld_out);
   count_launch();
   ZCHECK_LAUNCH();
   return ZEGGS_OK;
@@ -431,11 +442,11 @@ int gemm_f32_auto(int mode, int M, int N, int K, const float* A, int lda, const 
   if (rc == ZEGGS_CONV_NOT_TAKEN) return sgemm_launch(mode, M, N, K, A, lda, B, ldb, bias, C, ldc, act, accumulate, stream);
   if (rc) return rc;
   const dim3 tb(32, 8);
-  if (mode == 1) split_bf16_t_kernel<<<dim3(ceil_div(M, 32), ceil_div(Kp, 32)), tb, 0, stream>>>(A, K, M, lda, op.Ah, op.Al, Kp);
+  if (mode == 1) split_bf16_t_kernel<<<split_t_grid(M, Kp), tb, 0, stream>>>(A, K, M, lda, op.Ah, op.Al, Kp);
   else split_bf16_kernel<<<592, 256, 0, stream>>>(A, M, K, lda, op.Ah, op.Al, Kp);
   count_launch();
   if (mode == 0) split_bf16_kernel<<<592, 256, 0, stream>>>(B, N, K, ldb, op.Bh, op.Bl, Kp);
-  else split_bf16_t_kernel<<<dim3(ceil_div(N, 32), ceil_div(Kp, 32)), tb, 0, stream>>>(B, K, N, ldb, op.Bh, op.Bl, Kp);
+  else split_bf16_t_kernel<<<split_t_grid(N, Kp), tb, 0, stream>>>(B, K, N, ldb, op.Bh, op.Bl, Kp);
   count_launch();
   ZCHECK_LAUNCH();
   return tc_gemm_launch(M, N, K, op.Ah, op.Al, Kp, op.Bh, op.Bl, Kp, bias, C, ldc, act, accumulate, stream, op.ws, op.ws_bytes);
@@ -542,7 +553,7 @@ int conv_gemm_wgrad(const float* dpre, int N, const float* x, int B, int T, int 
   const int rc = plan_tc_operands(N, K, Mp, (double)M * N * K, true, &op);
   if (rc) return rc;
   const dim3 tb(32, 8);
-  split_bf16_t_kernel<<<dim3(ceil_div(N, 32), ceil_div(Mp, 32)), tb, 0, stream>>>(dpre, M, N, N, op.Ah, op.Al, Mp);
+  split_bf16_t_kernel<<<split_t_grid(N, Mp), tb, 0, stream>>>(dpre, M, N, N, op.Ah, op.Al, Mp);
   count_launch();
   im2col_split_t_kernel<<<dim3(ceil_div(C, 32), ceil_div(Mp, 128), k), tb, 0, stream>>>(x, B, T, C, k, pad, replicate, op.Bh, op.Bl, Mp);
   count_launch();
