@@ -390,10 +390,11 @@ int zeggs_normalize_rows(const float* x, const float* mean, const float* stdv, f
 
 /* Fused RAdam step over a flat fp32 parameter buffer (optimizers.py:31-99; weight_decay 0, degenerated_to_sgd), with every
  * step-dependent scalar in DEVICE memory, so that a captured CUDA graph can be replayed (gradients are multiplied by grad_scale first):
- * hyper[0..4] = lr, beta1, beta2, eps, grad_scale (inputs; the host rewrites them between replays when they change),
+ * hyper[0..4] = lr, beta1, beta2, eps, grad_scale as doubles (inputs; the host rewrites them between replays when they change),
  * hyper[5..7] = scratch written by the call; *step_count is the number of steps taken so far and is incremented by the call
- * (the rectification terms of optimizers.py:66-78 are evaluated on the device in double from *step_count + 1). */
-int zeggs_radam_step_dev(float* p, const float* g, float* m, float* v, size_t n, float* hyper, int* step_count, void* stream);
+ * (the rectification terms of optimizers.py:66-78 are evaluated on the device in double from *step_count + 1; 1 - beta is formed
+ * in double and each scalar the element pass uses is rounded to fp32 once, as torch rounds the reference's Python scalars). */
+int zeggs_radam_step_dev(float* p, const float* g, float* m, float* v, size_t n, double* hyper, int* step_count, void* stream);
 /* Dropout mask (u >= p) / (1 - p) with a counter-based generator: one pass instead of torch's rand / compare / cast / scale
  * (the Bernoulli draw of nn.Dropout, modules.py:263-270, :383-388, :551, :606).  Reproducible for a given seed. */
 int zeggs_dropout_mask(float* out, size_t n, float p, unsigned long long seed, void* stream);

@@ -521,24 +521,6 @@ def test_full_size_train_step_engines_agree(dev, decoder_engine):
     assert not bad, bad
 
 
-def test_dropout_mask_kernel(dev):
-    """zeggs_dropout_mask: values are 0 or 1/(1-p), keep fraction = 1-p within 4 sigma, reproducible under torch.manual_seed,
-    different for consecutive draws."""
-    from zeggs_b200 import ops
-    for p in (0.1, 0.2):
-        torch.manual_seed(5)
-        a = ops._drop_mask((64, 257, 33), p, dev)
-        b = ops._drop_mask((64, 257, 33), p, dev)
-        torch.manual_seed(5)
-        a2 = ops._drop_mask((64, 257, 33), p, dev)
-        n = a.numel()
-        keep = float((a > 0).float().mean())
-        assert torch.equal(a, a2) and not torch.equal(a, b)
-        vals = torch.unique(a).cpu().numpy()
-        assert len(vals) == 2 and vals[0] == 0.0 and abs(vals[1] - 1.0 / (1.0 - p)) <= 1e-6
-        assert abs(keep - (1.0 - p)) <= 4.0 * np.sqrt(p * (1.0 - p) / n)
-
-
 def test_label_style_z9_engines_agree(dev, decoder_engine):
     """configs_v2 geometry (one-hot label style, Z = 9 -> odd W_ih0 row stride A + H): the tensor-core engine against the fp32
     SIMT engine, window outputs <= 2e-2 * max(1, |ref|), parameter / speech gradient norms within 2e-2 relative."""

@@ -1,46 +1,50 @@
 // Fused multi-tensor RAdam (ZEGGS/optimizers.py:31-99) over one flat fp32 parameter buffer:
 // weight_decay = 0, degenerated_to_sgd = True (the configuration train.py:160 uses).  The step count and the
-// hyper-parameters live in device memory, so a captured CUDA graph can replay the step.  The rectification terms
-// depend only on the step count; one thread evaluates them in double, as the reference does in Python floats, and
-// the main kernel reads them back.  `grad_scale` folds the 1/world_size of the data-parallel all-reduce into the same pass.
+// hyper-parameters live in device memory, so a captured CUDA graph can replay the step.  The hyper-parameters are the host's
+// doubles: the reference forms 1 - beta and the rectification terms in Python floats and torch rounds each scalar to fp32 once,
+// so forming 1.0f - (float)beta2 instead would scale every v term by 1 - 1.3e-5 at beta2 = 0.999.  The rectification terms
+// depend only on the step count; one thread evaluates them in double and the main kernel reads them back.  `grad_scale` folds
+// the 1/world_size of the data-parallel all-reduce into the same pass.
 #include <math.h>
 #include "library.cuh"
 
 namespace zeggs {
 
-__global__ void radam_prep_kernel(float* __restrict__ hyper, int* __restrict__ step_count) {
+__global__ void radam_prep_kernel(double* __restrict__ hyper, int* __restrict__ step_count) {
   const int step = *step_count + 1;
   *step_count = step;
   const double lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2];
   const double b2t = pow(beta2, (double)step);
   const double n_max = 2.0 / (1.0 - beta2) - 1.0;
   const double n_sma = n_max - 2.0 * step * b2t / (1.0 - b2t);            // optimizers.py:66-68
-  double step_size; float adaptive;
+  double step_size, adaptive;
   if (n_sma >= 5.0) {
     step_size = sqrt((1.0 - b2t) * (n_sma - 4.0) / (n_max - 4.0) * (n_sma - 2.0) / n_sma * n_max / (n_max - 2.0)) /
                 (1.0 - pow(beta1, (double)step));                         // :72-76
-    adaptive = 1.f;
+    adaptive = 1.0;
   } else {
     step_size = 1.0 / (1.0 - pow(beta1, (double)step));                   // :77-78
-    adaptive = 0.f;
+    adaptive = 0.0;
   }
-  hyper[5] = (float)(step_size * lr);
+  hyper[5] = step_size * lr;
   hyper[6] = adaptive;
 }
 __global__ void radam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                                 size_t n, const float* __restrict__ hyper) {
-  const float beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], grad_scale = hyper[4], step_lr = hyper[5];
-  const bool adaptive = hyper[6] != 0.f;
+                                 size_t n, const double* __restrict__ hyper) {
+  // each scalar rounded to fp32 once, as torch rounds the Python scalars of optimizers.py:58-59, :89, :94
+  const float beta1 = (float)hyper[1], beta2 = (float)hyper[2], one_m_beta1 = (float)(1.0 - hyper[1]),
+              one_m_beta2 = (float)(1.0 - hyper[2]), eps = (float)hyper[3], grad_scale = (float)hyper[4], step_lr = (float)hyper[5];
+  const bool adaptive = hyper[6] != 0.0;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const float gi = g[i] * grad_scale;
-    const float vi = v[i] * beta2 + (1.0f - beta2) * gi * gi;     // optimizers.py:58
-    const float mi = m[i] * beta1 + (1.0f - beta1) * gi;          // :59
+    const float vi = v[i] * beta2 + one_m_beta2 * gi * gi;        // optimizers.py:58
+    const float mi = m[i] * beta1 + one_m_beta1 * gi;             // :59
     v[i] = vi; m[i] = mi;
     if (adaptive) p[i] = p[i] - step_lr * mi / (sqrtf(vi) + eps); // :88-89
     else p[i] = p[i] - step_lr * mi;                              // :94
   }
 }
-extern "C" int zeggs_radam_step_dev(float* p, const float* g, float* m, float* v, size_t n, float* hyper, int* step_count, void* stream) {
+extern "C" int zeggs_radam_step_dev(float* p, const float* g, float* m, float* v, size_t n, double* hyper, int* step_count, void* stream) {
   ZCHECK_ARG(p && g && m && v && hyper && step_count, "radam (device scalars): bad arguments");
   if (n == 0) return ZEGGS_OK;
   ScopedTimer tm("optimizer", (cudaStream_t)stream);

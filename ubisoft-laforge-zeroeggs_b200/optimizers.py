@@ -34,8 +34,9 @@ class RAdam(torch.optim.Optimizer):
         self._step = 0
         self.grad_scale = 1.0
         # step-dependent scalars live in DEVICE memory (zeggs_radam_step_dev) so a captured CUDA graph of the step can be replayed:
-        # hyper = [lr, beta1, beta2, eps, grad_scale, <scratch x3>], step_dev = steps taken so far (incremented by the kernel)
-        self.hyper = torch.zeros(8, dtype=torch.float32, device=dev)
+        # hyper = [lr, beta1, beta2, eps, grad_scale, <scratch x3>] in float64 (the kernel forms 1 - beta and the rectification terms
+        # from the host's doubles, as the reference does), step_dev = steps taken so far (incremented by the kernel)
+        self.hyper = torch.zeros(8, dtype=torch.float64, device=dev)
         self.step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
         self._hyper_host = None
 
@@ -45,7 +46,7 @@ class RAdam(torch.optim.Optimizer):
         g = self.param_groups[0]
         h = (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(self.grad_scale))
         if h != self._hyper_host:
-            self.hyper[:5].copy_(torch.tensor(h, dtype=torch.float32))
+            self.hyper[:5].copy_(torch.tensor(h, dtype=torch.float64))
             self._hyper_host = h
 
     def zero_grad(self, set_to_none=False):
