@@ -495,6 +495,32 @@ typedef struct {
 size_t zeggs_masked_moments_workspace_bytes(long long n_sel, int total_width);
 int zeggs_masked_moments(const zeggs_moments_args* a, void* stream);
 
+/* Style embedding space statistics (zeggs_b200.style_space; beyond the reference): float64 moments of N float32 rows X [N, Z], row
+ * r in group group[r] (int32, 0 <= group[r] < G; not checked on the device: a row outside that range is left out of every group sum
+ * and count, and ops.embedding_moments checks the ids before the call).  Outputs
+ *   group_sum [G, Z] f64    sum of the rows of each group          group_count [G] int64   rows of each group
+ *   mean [Z] f64            (sum over groups of group_sum) / N     cov [Z, Z] f64          Xc^T Xc / (N - 1), Xc = X - mean
+ * Two passes (the mean, then the centred products: no E[xx^T] - mu mu^T cancellation) and a fixed reduction order, so two calls on
+ * the same input give the same bits.  The rows are cut into S slices of R consecutive rows,
+ *   nb = ceil(Z / 64), tiles = nb (nb + 1) / 2, S0 = min(ceil(N / 256), max(1, 512 / tiles)), R = ceil(N / S0), S = ceil(N / R),
+ * each slice summed in row order by one CTA, and the S partials added in slice order (group sums: then the groups in order for the
+ * mean).  cov is exactly symmetric; with N = 1 it is 0/0 = NaN, as numpy.cov gives.  1 <= Z <= ZEGGS_EMBED_MAX_Z,
+ * 1 <= G <= ZEGGS_EMBED_MAX_GROUPS (the per-slice group sums of one CTA live in shared memory). */
+#define ZEGGS_EMBED_MAX_GROUPS 128
+#define ZEGGS_EMBED_MAX_Z 16384
+typedef struct {
+  long long N;
+  int Z, G;
+  const float* X;
+  const int* group;
+  double *mean, *cov, *group_sum;
+  long long* group_count;
+  void* workspace;
+  size_t workspace_bytes;
+} zeggs_embedding_moments_args;
+size_t zeggs_embedding_moments_workspace_size(long long N, int Z, int G);   /* 0 when N, Z or G is out of range */
+int zeggs_embedding_moments(const zeggs_embedding_moments_args* a, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Rate conversion of a WAV file's samples to 16 kHz mono.  Replaces the SoX step of the reference's read_wavfile
  * (audio/audio_files.py:52-78 reformat_and_trim_wav_file: `rate -h`, `channels 1`, 32-bit output; :88-163 read_wavfile), which

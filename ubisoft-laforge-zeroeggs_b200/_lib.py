@@ -125,6 +125,12 @@ BvhFormatArgs = _struct("BvhFormatArgs", ints=("T", "J", "in_f64", "max_flagged"
                         tail=[("positions", C.c_void_p), ("rotations", C.c_void_p), ("seq", C.c_void_p), ("out", C.c_void_p),
                               ("out_capacity", C.c_longlong), ("row_start", C.c_void_p), ("flagged", C.c_void_p), ("status", C.c_void_p),
                               ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
+EMBED_MAX_GROUPS = 128
+EMBED_MAX_Z = 16384
+EmbeddingMomentsArgs = _struct("EmbeddingMomentsArgs", tail=[("N", C.c_longlong), ("Z", C.c_int), ("G", C.c_int), ("X", C.c_void_p),
+                                                             ("group", C.c_void_p), ("mean", C.c_void_p), ("cov", C.c_void_p),
+                                                             ("group_sum", C.c_void_p), ("group_count", C.c_void_p),
+                                                             ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)])
 
 
 # every symbol include/zeggs_b200.h declares: (name, restype, argtypes)
@@ -138,7 +144,7 @@ def struct_mirrors():
             "zeggs_anim_features_args": AnimFeaturesArgs, "zeggs_spline_args": SplineArgs, "zeggs_moments_args": MomentsArgs,
             "zeggs_resample_args": ResampleArgs, "zeggs_decoder_film_fwd_args": DecoderFilmFwdArgs,
             "zeggs_decoder_film_bwd_args": DecoderFilmBwdArgs, "zeggs_bvh_parse_args": BvhParseArgs,
-            "zeggs_bvh_format_args": BvhFormatArgs}
+            "zeggs_bvh_format_args": BvhFormatArgs, "zeggs_embedding_moments_args": EmbeddingMomentsArgs}
 
 
 SYMBOLS = [
@@ -208,6 +214,8 @@ SYMBOLS = [
     ("zeggs_spline_resample", C.c_int, [C.POINTER(SplineArgs), C.c_void_p]),
     ("zeggs_masked_moments_workspace_bytes", C.c_size_t, [C.c_longlong, C.c_int]),
     ("zeggs_masked_moments", C.c_int, [C.POINTER(MomentsArgs), C.c_void_p]),
+    ("zeggs_embedding_moments_workspace_size", C.c_size_t, [C.c_longlong, C.c_int, C.c_int]),
+    ("zeggs_embedding_moments", C.c_int, [C.POINTER(EmbeddingMomentsArgs), C.c_void_p]),
     ("zeggs_resample", C.c_int, [C.POINTER(ResampleArgs), C.c_void_p]),
     ("zeggs_bvh_parse_motion_workspace_size", C.c_size_t, [C.c_longlong, C.c_int]),
     ("zeggs_bvh_parse_motion", C.c_int, [C.POINTER(BvhParseArgs), C.c_void_p]),

@@ -163,6 +163,7 @@ extern "C" size_t zeggs_struct_size(const char* name) {
   ZS(zeggs_pose_post_args) ZS(zeggs_gather_args) ZS(zeggs_style_enc_gru_args) ZS(zeggs_style_enc_gru_grads)
   ZS(zeggs_anim_features_args) ZS(zeggs_spline_args) ZS(zeggs_moments_args) ZS(zeggs_resample_args)
   ZS(zeggs_decoder_film_fwd_args) ZS(zeggs_decoder_film_bwd_args) ZS(zeggs_bvh_parse_args) ZS(zeggs_bvh_format_args)
+  ZS(zeggs_embedding_moments_args)
 #undef ZS
   return 0;
 }

@@ -843,3 +843,31 @@ def masked_moments(groups, rows):
         a.width[i] = int(s.shape[1])
     _lib.check(l.zeggs_masked_moments(a, _lib.stream_ptr()), "zeggs_masked_moments")
     return mean, std, gstd
+
+
+def embedding_moments(X, group, n_groups):
+    """float64 statistics of embedding rows (zeggs_embedding_moments): X [N, Z] float32 CUDA tensor, group [N] ints in 0..n_groups-1
+    -> (mean [Z], cov [Z, Z] = Xc^T Xc / (N - 1), group_sum [n_groups, Z] f64, group_count [n_groups] int64), CUDA tensors.  Two
+    passes and a fixed reduction order: the same input gives the same bits on every call."""
+    if not X.is_cuda:
+        raise _lib.ZeggsError("embedding_moments runs on CUDA tensors only (no CPU fallback)")
+    if X.dim() != 2:
+        raise _lib.ZeggsError(f"embedding_moments: X must be [N, Z], got shape {tuple(X.shape)}")
+    N, Z, G = int(X.shape[0]), int(X.shape[1]), int(n_groups)
+    dev = X.device
+    X = X.to(torch.float32).contiguous()
+    group = torch.as_tensor(group, device=dev).to(torch.int32).contiguous()
+    if group.shape != (N,):
+        raise _lib.ZeggsError(f"embedding_moments: group has shape {tuple(group.shape)}, X has {N} rows")
+    if N and not (0 <= int(group.min()) and int(group.max()) < G):
+        raise _lib.ZeggsError(f"embedding_moments: group ids must lie in 0..{G - 1}")
+    l = _lib.lib()
+    wsb = l.zeggs_embedding_moments_workspace_size(N, Z, G)   # 0 for a shape the call below refuses, naming the limit
+    ws = WS.get("embedding_moments", max(wsb, 1), dev)
+    f64 = dict(dtype=torch.float64, device=dev)
+    mean, cov, gsum = torch.empty(Z, **f64), torch.empty((Z, Z), **f64), torch.empty((G, Z), **f64)
+    gcount = torch.empty(G, dtype=torch.int64, device=dev)
+    a = _lib.EmbeddingMomentsArgs(N=N, Z=Z, G=G, X=_lib.ptr(X), group=_lib.ptr(group), mean=mean.data_ptr(), cov=cov.data_ptr(),
+                                  group_sum=gsum.data_ptr(), group_count=gcount.data_ptr(), workspace=ws.data_ptr(), workspace_bytes=wsb)
+    _lib.check(l.zeggs_embedding_moments(a, _lib.stream_ptr()), "zeggs_embedding_moments")
+    return mean, cov, gsum, gcount
